@@ -244,11 +244,11 @@ int launch_idct(jxlgpu_ctx* ctx, uint32_t row0, uint32_t row1, uint32_t need_y0,
     if (fused) return;  // (the fused kernel transforms the 8x8 class itself)
     bool tma = ctx->idct8_tma;
     for (int c = 0; c < 3; c++) tma = tma && (uintptr_t)P.coeff[c] % 16 == 0;
-    if (tma) {  // coefficients staged by the bulk-copy unit one item ahead (3 CTAs per SM)
-      int grid = ctx->num_sms * 3;
-      if (grid > grid8) grid = grid8;
-      if (P.ac_is32) idct8_tma_kernel<true><<<grid, kSmallWarpsPerCta * 32, kTma8SmemBytes, s>>>(P);
-      else idct8_tma_kernel<false><<<grid, kSmallWarpsPerCta * 32, kTma8SmemBytes, s>>>(P);
+    if (tma) {  // coefficients staged by the bulk-copy unit one item ahead (2 CTAs of 16 warps per SM)
+      int grid = ctx->num_sms * 2;
+      if ((uint32_t)grid > px_blocks / 64u + 1u) grid = (int)(px_blocks / 64u + 1u);  // 64 blocks per CTA round
+      if (P.ac_is32) idct8_tma_kernel<true><<<grid, kTma8Warps * 32, kTma8SmemBytes, s>>>(P);
+      else idct8_tma_kernel<false><<<grid, kTma8Warps * 32, kTma8SmemBytes, s>>>(P);
       return;
     }
     if (P.ac_is32) idct8_kernel<true><<<grid8, kSmallWarpsPerCta * 32, 0, s>>>(P);

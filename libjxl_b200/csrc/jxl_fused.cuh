@@ -103,6 +103,7 @@ __device__ __forceinline__ int mod_n(int s, int n) { s %= n; return s < 0 ? s + 
 struct Block8ToRing {
   static constexpr int kPitch = kTRow;
   static constexpr bool kGuardPx = true;
+  static constexpr bool kDctRows = false;
   float* base;  // ring address of (row 0 of the block row, channel 0, first column of the block)
   __device__ __forceinline__ float* px(int c) const { return base + c * kTPitch; }
   __device__ __forceinline__ void dct_col(int c, int l, const float* u, bool active) const {
@@ -111,7 +112,6 @@ struct Block8ToRing {
 #pragma unroll
       for (int y = 0; y < 8; y++) o[y * kTRow] = u[y];
     }
-    __syncwarp();
   }
   __device__ __forceinline__ void finish(int, int, bool) const { __syncwarp(); }
 };
@@ -652,8 +652,7 @@ fused_tile_kernel(const __grid_constant__ FrameDev P, char* __restrict__ out, si
           const uint4 rec = recs[rank];
           const int kind = (int)(rec.x & 0xffu), bxl = (int)((rec.x >> 8) & 0xffu);
           uint32_t* stg = scratch + rank * kTScratchWords;
-          float* co = reinterpret_cast<float*>(stg);
-          float* tmp = co + 96;
+          float* scr = reinterpret_cast<float*>(stg);
           Block8ToRing ro;
           ro.base = rings + (size_t)((B % 3) * 8) * kTRow + bxl * 8;
           float val[3][8];
@@ -669,12 +668,10 @@ fused_tile_kernel(const __grid_constant__ FrameDev P, char* __restrict__ out, si
             vb.sb = s * P.b_dm;
             vb.x_cc = P.cfl_base_x + (float)(int)(int8_t)(rec.w & 0xffu) * P.cfl_scale;
             vb.b_cc = P.cfl_base_b + (float)(int)(int8_t)((rec.w >> 8) & 0xffu) * P.cfl_scale;
-            int qx[8], qy[8], qb[8];
             constexpr int kChWords = I32 ? 64 : 32;
-            load_row8_smem<I32>(stg + kChWords, l * 8, qy);
-            load_row8_smem<I32>(stg, l * 8, qx);
-            load_row8_smem<I32>(stg + 2 * kChWords, l * 8, qb);
-            block8_dequant_row(P, kind, vb, l, qx, qy, qb, val);
+            const bool col = kind == 0;  // (per slot: the slots of an item may hold different kinds)
+            block8_dequant(P, kind, vb, l, col,
+                           [&](int c, int* q) { load_lane8_smem<I32>(stg + c * kChWords, l, col, q); }, val);
           } else {
 #pragma unroll
             for (int c = 0; c < 3; c++)
@@ -706,7 +703,7 @@ fused_tile_kernel(const __grid_constant__ FrameDev P, char* __restrict__ out, si
               }
               continue;
             }
-            block8_transform(kc, act, val, l, co, tmp, ro);
+            block8_transform(kc, act, val, l, scr, ro);
           }
           fence_async_smem();  // the scratch is the TMA destination of the next block row
         } else {
