@@ -263,7 +263,10 @@ JXLGPU_API int jxlgpu_frame_finish(jxlgpu_ctx* ctx, void* out, size_t out_stride
 /* ---- device-resident entry points (bench / multi-GPU plumbing; pointers are DEVICE) ---- */
 
 /* Use coefficient planes that already live in HBM: dev_coeff[c] = [num_groups][65536]
- * elements of the frame's ac_type.  Marks every group as submitted. */
+ * elements of the frame's ac_type.  Marks every group as submitted.  Each plane must be aligned to
+ * the element size (2 bytes for int16, 4 for int32): jxlgpu_render_device / jxlgpu_frame_finish
+ * return JXLGPU_ERR_INVALID_ARGUMENT otherwise, before enqueuing anything.  16-byte aligned planes
+ * select the bulk-copy 8x8 kernel; others are read with ordinary loads, which is slower. */
 JXLGPU_API int jxlgpu_set_device_coefficients(jxlgpu_ctx* ctx, const void* const dev_coeff[3]);
 /* Enqueue the whole hot path on `cuda_stream` (a cudaStream_t, 0 = context stream) writing
  * the band to dev_out (device pointer or NULL for the context's own buffer). No host sync. */

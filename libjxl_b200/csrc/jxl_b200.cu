@@ -187,6 +187,17 @@ bool fused_chain(uint32_t mask) {
     default: return false;
   }
 }
+// The kernels load whole elements from the coefficient planes: a caller's device-resident planes
+// (jxlgpu_set_device_coefficients) must be aligned to the frame's element size.
+bool coeff_planes_aligned(jxlgpu_ctx* ctx) {
+  for (int c = 0; c < 3; c++)
+    if ((uintptr_t)ctx->P.coeff[c] % ctx->elem_size) {
+      ctx->last_error = "coefficient planes must be aligned to the element size of the frame's ac_type";
+      return false;
+    }
+  return true;
+}
+
 bool use_fused(const jxlgpu_ctx* ctx) {
   const FrameDev& P = ctx->P;
   if (!ctx->allow_fused || ctx->force_generic_filter || !fused_chain(P.stage_mask) || P.mc || P.ups || P.noise || P.ycbcr) return false;
@@ -1016,6 +1027,7 @@ int jxlgpu_render_device(jxlgpu_ctx* ctx, void* dev_out, size_t out_stride_bytes
   if (!ctx->in_frame) return JXLGPU_ERR_STATE;
   CU(cudaSetDevice(ctx->device));
   std::lock_guard<std::mutex> lk(ctx->mu);
+  if (!coeff_planes_aligned(ctx)) return JXLGPU_ERR_INVALID_ARGUMENT;
   cudaStream_t s = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
   if (cuda_stream) {  // side info was uploaded on the context stream
     CU(cudaEventRecord(ctx->ev_ext, ctx->stream));
@@ -1129,6 +1141,7 @@ int jxlgpu_frame_finish(jxlgpu_ctx* ctx, void* out, size_t out_stride_bytes) {
         ctx->last_error = "missing group";
         return JXLGPU_ERR_STATE;
       }
+    if (!coeff_planes_aligned(ctx)) return JXLGPU_ERR_INVALID_ARGUMENT;
     int rc = pump(ctx, true);  // whatever the scheduler still holds back, and device-resident coefficients
     if (rc) return rc;
     for (uint32_t g = ctx->band_row0; g < ctx->band_row1; g++)

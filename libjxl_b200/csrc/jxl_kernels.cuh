@@ -643,15 +643,19 @@ __device__ __forceinline__ void load_row8_smem(const void* block, int elem, int*
 
 // The 8 coefficients lane l of an 8x8-class block owns in one channel: column l for DCT8x8 (`col`: its first
 // 1-D pass runs down the columns in registers), row l for the specials.
-//   load_lane8: from the channel plane in HBM (e0 = element index of coefficient 0)
+//   load_lane8: from the channel plane in HBM (e0 = element index of coefficient 0); a row is two / one 16-byte
+//     loads when the plane is 16-byte aligned (`vec`), element loads otherwise
 //   load_lane8_smem: from the block staged in SHARED memory
 template <bool I32>
-__device__ __forceinline__ void load_lane8(const void* plane, size_t e0, int l, bool col, int* q) {
+__device__ __forceinline__ void load_lane8(const void* plane, size_t e0, int l, bool col, bool vec, int* q) {
   if (col) {
 #pragma unroll
     for (int k = 0; k < 8; k++) q[k] = load_q<I32>(plane, e0 + k * 8 + l);
-  } else {
+  } else if (vec) {
     load_row8<I32>(plane, e0 + (size_t)l * 8, q);
+  } else {
+#pragma unroll
+    for (int k = 0; k < 8; k++) q[k] = load_q<I32>(plane, e0 + (size_t)l * 8 + k);
   }
 }
 template <bool I32>
@@ -1051,9 +1055,10 @@ __device__ __forceinline__ void block8_transform(int kind, bool active, const fl
 // Phase A: lane l loads its column (DCT8x8) or row (the specials) of all three channels and dequantises
 // them in registers (CfL needs Y next to X and B anyway).
 // Phase B: the strategy's transform (block8_transform).
+// vec: the coefficient planes are 16-byte aligned (rows of the specials as vector loads, see load_lane8).
 template <bool I32>
 __device__ __forceinline__ void block8_item(const FrameDev& P, int kind, uint4 entry, bool active,
-                                            uint4 entry_next, bool next_active, float* sm) {
+                                            uint4 entry_next, bool next_active, bool vec, float* sm) {
   const int lane = threadIdx.x & 31;
   const int slot = lane >> 3, l = lane & 7;
   // Inactive slots (tail of a list) run the same instruction stream on scratch data so that
@@ -1065,7 +1070,7 @@ __device__ __forceinline__ void block8_item(const FrameDev& P, int kind, uint4 e
     vb = make_ctx(P, entry);
     const bool col = kind == 0;
     block8_dequant(P, kind, vb, l, col,
-                   [&](int c, int* q) { load_lane8<I32>(P.coeff[c], vb.cbase, l, col, q); }, val);
+                   [&](int c, int* q) { load_lane8<I32>(P.coeff[c], vb.cbase, l, col, vec, q); }, val);
   } else {
     vb = VarblockCtx{};
 #pragma unroll
@@ -1104,13 +1109,15 @@ __device__ __forceinline__ int small_slots(int s) {
   return w == 1 ? 4 : (w == 2 ? 2 : 1);
 }
 
-// 8x8-class strategies (DCT, IDENTITY, DCT2X2, DCT4X4, DCT4X8, DCT8X4, AFV0-3).
+// 8x8-class strategies (DCT, IDENTITY, DCT2X2, DCT4X4, DCT4X8, DCT8X4, AFV0-3).  Takes any element-aligned
+// coefficient planes (device-resident planes of a caller need not be 16-byte aligned).
 template <bool I32>
 __global__ void __launch_bounds__(kSmallWarpsPerCta * 32, 4) idct8_kernel(const __grid_constant__ FrameDev P) {
   __shared__ __align__(16) float smem[kSmallWarpsPerCta * 1056];
   float* sm = smem + (threadIdx.x >> 5) * 1056;
   const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
+  const bool vec = (((uintptr_t)P.coeff[0] | (uintptr_t)P.coeff[1] | (uintptr_t)P.coeff[2]) & 15u) == 0;
   const int order[10] = {0, 2, 12, 13, 1, 3, 14, 15, 16, 17};
   uint32_t base = 0;
 #pragma unroll 1
@@ -1130,7 +1137,7 @@ __global__ void __launch_bounds__(kSmallWarpsPerCta * 32, 4) idct8_kernel(const 
         const uint32_t nx = (it + nwarps) * 4 + slot;  // the record of this warp's next item is fetched now
         const bool nact = (it + nwarps) < items && nx < count;
         const uint4 next = nact ? __ldg(list + nx) : zero;
-        block8_item<I32>(P, s, cur, act, next, nact, sm);
+        block8_item<I32>(P, s, cur, act, next, nact, vec, sm);
         cur = next;
         act = nact;
       }

@@ -112,8 +112,22 @@ inline unsigned __ballot_sync(unsigned, bool pred) {
 }
 inline int __popc(unsigned v) { return __builtin_popcount(v); }
 inline float __uint_as_float(unsigned u) { float f; memcpy(&f, &u, 4); return f; }
+// A load whose address breaks alignof(T) is a misaligned-address fault on the GPU; x86 does not care, so
+// __ldg counts them (emu_misaligned_loads) and copies bytewise instead of faulting.
+namespace emu {
+inline std::atomic<uint64_t> g_misaligned_loads{0};
+}
 template <typename T>
-inline T __ldg(const T* p) { return *p; }
+inline T __ldg(const T* p) {
+  if ((uintptr_t)p % alignof(T)) emu::g_misaligned_loads.fetch_add(1, std::memory_order_relaxed);
+  T v;
+  memcpy(&v, p, sizeof(T));
+  return v;
+}
+// the number of misaligned __ldg loads since the last reset (reset != 0: start counting from zero again)
+extern "C" __attribute__((visibility("default"), used)) inline uint64_t emu_misaligned_loads(int reset) {
+  return reset ? emu::g_misaligned_loads.exchange(0) : emu::g_misaligned_loads.load();
+}
 template <typename T>
 inline T atomicAdd(T* p, T v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
 inline int __float2int_rn(float x) { return (int)lrintf(x); }

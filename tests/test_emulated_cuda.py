@@ -396,6 +396,65 @@ def test_emulated_argument_validation(emu_pipe):
     assert lib.jxlgpu_submit_group(emu_pipe._h, 0, 0, ptrs, 1000) == abi.ERR_STATE
 
 
+def planes_at_offset(coeffs, offset):
+    """The three coefficient planes, each in its own byte buffer starting `offset` bytes past a 16-byte boundary
+    (what a caller's sub-allocation can hand to jxlgpu_set_device_coefficients).  Returns (buffers, addresses)."""
+    bufs, ptrs = [], []
+    for c in range(3):
+        src = np.ascontiguousarray(coeffs[c]).view(np.uint8).ravel()
+        buf = np.zeros(src.size + 32, np.uint8)
+        o = (-buf.ctypes.data) % 16 + offset
+        buf[o:o + src.size] = src
+        bufs.append(buf)
+        ptrs.append(buf.ctypes.data + o)
+    return bufs, ptrs
+
+
+@pytest.mark.timeout(900)
+def test_emulated_unaligned_device_planes(emu_pipe):
+    """Device-resident planes that are element-aligned but not 16-byte aligned go to idct8_kernel (the bulk copies of
+    idct8_tma_kernel need 16 bytes); it must load them without one vector load at a misaligned address (the shim
+    counts what the GPU would fault on) and give the oracle's pixels.  Planes that are not even element-aligned are
+    refused before anything is launched."""
+    lib = pipeline.lib()
+    lib.emu_misaligned_loads.restype, lib.emu_misaligned_loads.argtypes = C.c_uint64, [C.c_int]
+    frames = [wl.synthetic_frame(96, 64, seed=5, strategies="0,1,2,3,12,13,14,15,16,17"),   # the 8x8 class only
+              wl.synthetic_frame(264, 136, seed=6)]                                         # all strategies
+    for ac_type, offsets in ((abi.AC_INT16, (2, 8)), (abi.AC_INT32, (4, 8))):
+        for desc, coeffs in frames:
+            desc.ac_type = ac_type
+            coeffs = coeffs.astype(np.int16 if ac_type == abi.AC_INT16 else np.int32)
+            desc.stage_mask, desc.out_format = abi.STAGE_EXPLICIT | 0, abi.OUT_PLANAR_F32   # after the transforms
+            want = oracle(desc, coeffs)
+            for off in offsets:
+                bufs, ptrs = planes_at_offset(coeffs, off)
+                out = np.full(desc.out_shape(), np.nan, np.float32)
+                emu_pipe.set_device_coefficients(ptrs)
+                try:
+                    emu_pipe.frame_begin(desc)
+                    lib.emu_misaligned_loads(1)
+                    emu_pipe.render_device(out.ctypes.data, desc.out_row_bytes)
+                    misaligned = lib.emu_misaligned_loads(0)
+                finally:
+                    emu_pipe.set_device_coefficients(None)
+                assert misaligned == 0, (desc.xsize, ac_type, off, misaligned)
+                assert same(out, want), (desc.xsize, ac_type, off)
+    desc, coeffs = frames[0]                       # (int32 after the loop) at +2: not a multiple of 4 bytes
+    assert desc.ac_type == abi.AC_INT32
+    bufs, ptrs = planes_at_offset(coeffs.astype(np.int32), 2)
+    out = np.zeros(desc.out_shape(), np.float32)
+    emu_pipe.set_device_coefficients(ptrs)
+    try:
+        emu_pipe.frame_begin(desc)
+        before = emu_pipe.launch_count()
+        with pytest.raises(pipeline.JxlGpuError):
+            emu_pipe.render_device(out.ctypes.data, desc.out_row_bytes)
+        assert lib.jxlgpu_frame_finish(emu_pipe._h, None, 0) == abi.ERR_INVALID_ARGUMENT   # the host-side finish too
+        assert emu_pipe.launch_count() == before
+    finally:
+        emu_pipe.set_device_coefficients(None)
+
+
 def epf_engaged_frame(w, h, seed, gab=1, epf_iters=3):
     """A synthetic frame whose EPF weights are non-zero (raw_quant 1, sharpness 7 puts sigma above
     kMinSigma; smooth, small coefficients keep the SADs small).  synthetic_frame's random quantisers
