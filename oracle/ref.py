@@ -53,6 +53,22 @@ class RefFrameInfo(C.Structure):
     ]
 
 
+class RefFrameParams(C.Structure):
+    """ref_frame_set_params: frame-header / image-metadata values written into an opened frame."""
+    _fields_ = [
+        ("x_dm_multiplier", C.c_float), ("b_dm_multiplier", C.c_float),
+        ("quant_biases", C.c_float * 4),
+        ("cfl_base_x", C.c_float), ("cfl_base_b", C.c_float), ("color_factor", C.c_uint32),
+        ("gab_weights", C.c_float * 6),
+        ("epf_sharp_lut", C.c_float * 8),
+        ("epf_channel_scale", C.c_float * 3),
+        ("epf_quant_mul", C.c_float), ("epf_pass0_sigma_scale", C.c_float),
+        ("epf_pass2_sigma_scale", C.c_float), ("epf_border_sad_mul", C.c_float),
+        ("inverse_opsin_matrix", C.c_float * 9),
+        ("opsin_biases", C.c_float * 3),
+    ]
+
+
 PLANE_AC_STRATEGY, PLANE_RAW_QUANT, PLANE_SHARPNESS, PLANE_YTOX, PLANE_YTOB = 0, 1, 2, 3, 4
 PLANE_DC, PLANE_SIGMA, PLANE_DEQUANT, PLANE_COEFFS, PLANE_DECODED = 5, 6, 7, 8, 9
 
@@ -66,6 +82,12 @@ _variant = "default"
 
 def available(variant: str = "default") -> bool:
     return _SO[variant].exists()
+
+
+def can_set_params() -> bool:
+    """Whether the selected harness build has ref_frame_set_params (Frame.set_params).  A prebuilt oracle/_ref
+    made from an older harness, on a machine without the reference sources to rebuild it, does not."""
+    return hasattr(lib(), "ref_frame_set_params")
 
 
 def use_variant(variant: str) -> None:
@@ -90,6 +112,8 @@ def lib():
         L.ref_frame_raw_coeffs.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]
         L.ref_frame_close.argtypes = [C.c_void_p]
         L.ref_frame_info.argtypes = [C.c_void_p, C.POINTER(RefFrameInfo)]
+        if hasattr(L, "ref_frame_set_params"):   # (absent from a harness built before it existed)
+            L.ref_frame_set_params.argtypes = [C.c_void_p, C.POINTER(RefFrameParams)]
         L.ref_frame_get_plane.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]
         L.ref_frame_render.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_double)]
         L.ref_decode_native.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_size_t,
@@ -204,6 +228,7 @@ class Frame:
     def __init__(self, data: bytes, threads: int = 1, storage: int = 0):
         """storage 1: the reference's entropy decoder writes through integration/pinned_ac_image.h
         (group-major layout) instead of its own ACImageT."""
+        self.h = None
         self.h = lib().ref_frame_open_storage(data, len(data), threads, storage)
         if not self.h:
             raise RuntimeError("ref_frame_open failed (frame not eligible for the hot path?)")
@@ -219,6 +244,24 @@ class Frame:
         if rc:
             raise RuntimeError(f"ref_frame_bind_gpu_frame rc={rc}")
         return s
+
+    def set_params(self, hdr: dict) -> None:
+        """Write a header set (jxl_workload.header_params: the HEADER_FIELDS plus color_factor) into the opened
+        frame as if its bitstream had carried it; the sigma image is recomputed.  `info` (and so dump(),
+        desc_from_dump and bind_gpu_frame) then reports the new values."""
+        if not can_set_params():
+            raise RuntimeError(f"{_SO[_variant]} predates ref_frame_set_params: rebuild it with `python oracle/build_ref.py`")
+        p = RefFrameParams()
+        for name, _ in RefFrameParams._fields_:
+            v = hdr[name]
+            if hasattr(getattr(p, name), "__len__"):
+                getattr(p, name)[:] = [float(x) for x in v]
+            else:
+                setattr(p, name, v)
+        rc = lib().ref_frame_set_params(self.h, C.byref(p))
+        if rc:
+            raise RuntimeError(f"ref_frame_set_params rc={rc}")
+        lib().ref_frame_info(self.h, C.byref(self.info))
 
     def raw_group_major_coeffs(self) -> np.ndarray:
         """storage 1 only: the allocation itself, viewed as (num_groups, 3, 65536) -- exactly the host

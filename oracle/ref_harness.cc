@@ -26,10 +26,12 @@
 #include <jxl/thread_parallel_runner.h>
 
 #include <chrono>
+#include <cmath>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <limits>
 #include <memory>
 #include <vector>
 
@@ -596,6 +598,128 @@ REF_API int ref_frame_info(void* h, RefFrameInfo* o) {
       o->dequant_offsets[k * 3 + c] =
           sh.matrices.Matrix(static_cast<AcStrategyType>(k), c) - base;
   return 0;
+}
+
+// ---------------------------------------------------------------------------
+// (3b) override the frame-header / image-metadata parameters of an opened frame,
+// as if the bitstream had carried them: the LoopFilter's custom Gaborish / EPF
+// fields, the qm-scale dequantisation multipliers, the DC colour-correlation
+// header (base correlations, colour factor) and the metadata's opsin inverse
+// matrix (already x 255 / intensity_target), opsin and quantisation biases.
+// The sigma image is recomputed with the reference's ComputeSigma, because the
+// EPF fields feed it.  Values must be ones the bitstream can carry: the base
+// correlations go through the reference's own F16 decoder.
+// ---------------------------------------------------------------------------
+struct RefFrameParams {
+  float x_dm_multiplier, b_dm_multiplier;
+  float quant_biases[4];
+  float cfl_base_x, cfl_base_b;
+  uint32_t color_factor;
+  float gab_weights[6];                     // x1 x2 y1 y2 b1 b2
+  float epf_sharp_lut[8];
+  float epf_channel_scale[3];
+  float epf_quant_mul, epf_pass0_sigma_scale, epf_pass2_sigma_scale, epf_border_sad_mul;
+  float inverse_opsin_matrix[9];
+  float opsin_biases[3];
+};
+
+namespace {
+
+// LSB-first bit packing, the order BitReader reads in
+struct BitPacker {
+  std::vector<uint8_t> bytes = std::vector<uint8_t>(32, 0);
+  size_t pos = 0;
+  void Put(uint32_t v, size_t n) {
+    for (size_t i = 0; i < n; i++, pos++)
+      if ((v >> i) & 1) bytes[pos / 8] |= static_cast<uint8_t>(1u << (pos % 8));
+  }
+};
+
+// IEEE binary16 bits of f; false when f is not exactly representable (no inf / NaN in F16 fields)
+bool HalfBits(float f, uint32_t* bits) {
+  const uint32_t sign = std::signbit(f) ? 0x8000u : 0u;
+  const float a = std::fabs(f);
+  if (a == 0.0f) { *bits = sign; return true; }
+  int e;
+  std::frexp(a, &e);                        // a = m * 2^e, m in [0.5, 1)
+  const int biased = e - 1 + 15;
+  if (biased > 30) return false;
+  const float unit = std::ldexp(1.0f, (biased >= 1 ? e - 1 : -14) - 10);   // value of one mantissa step
+  const float steps = a / unit;
+  const uint32_t m = static_cast<uint32_t>(steps);
+  if (static_cast<float>(m) != steps) return false;
+  *bits = biased >= 1 ? sign | (static_cast<uint32_t>(biased) << 10) | (m - 1024) : sign | m;
+  return true;
+}
+
+Status SetParamsImpl(RefFrame* f, const RefFrameParams& p) {
+  LoopFilter& lf = f->frame_header->loop_filter;
+  lf.gab_custom = true;
+  lf.gab_x_weight1 = p.gab_weights[0]; lf.gab_x_weight2 = p.gab_weights[1];
+  lf.gab_y_weight1 = p.gab_weights[2]; lf.gab_y_weight2 = p.gab_weights[3];
+  lf.gab_b_weight1 = p.gab_weights[4]; lf.gab_b_weight2 = p.gab_weights[5];
+  lf.epf_sharp_custom = true;
+  memcpy(lf.epf_sharp_lut, p.epf_sharp_lut, sizeof(lf.epf_sharp_lut));
+  lf.epf_weight_custom = true;
+  memcpy(lf.epf_channel_scale, p.epf_channel_scale, sizeof(lf.epf_channel_scale));
+  lf.epf_sigma_custom = true;
+  lf.epf_quant_mul = p.epf_quant_mul;
+  lf.epf_pass0_sigma_scale = p.epf_pass0_sigma_scale;
+  lf.epf_pass2_sigma_scale = p.epf_pass2_sigma_scale;
+  lf.epf_border_sad_mul = p.epf_border_sad_mul;
+
+  PassesDecoderState* ds = f->dec_state.get();
+  ds->x_dm_multiplier = p.x_dm_multiplier;
+  ds->b_dm_multiplier = p.b_dm_multiplier;
+  OpsinParams& op = ds->output_encoding_info.opsin_params;
+  for (int i = 0; i < 9; i++)
+    for (int lane = 0; lane < 4; lane++) op.inverse_opsin_matrix[i * 4 + lane] = p.inverse_opsin_matrix[i];
+  for (int c = 0; c < 3; c++) {
+    op.opsin_biases[c] = p.opsin_biases[c];
+    op.opsin_biases_cbrt[c] = cbrtf(p.opsin_biases[c]);
+  }
+  memcpy(op.quant_biases, p.quant_biases, sizeof(op.quant_biases));
+
+  // the DC colour-correlation header: not all default, colour factor (U32), two F16 base correlations, and
+  // the frame's own DC correlations again (RecomputeDCFactors keeps them)
+  ColorCorrelationMap& cmap = ds->shared_storage.cmap;
+  const ColorCorrelation& cc = cmap.base();
+  BitPacker bits;
+  bits.Put(0, 1);
+  const uint32_t cf = p.color_factor;
+  if (cf == kDefaultColorFactor) bits.Put(0, 2);
+  else if (cf == 256) bits.Put(1, 2);
+  else if (cf >= 2 && cf < 258) { bits.Put(2, 2); bits.Put(cf - 2, 8); }
+  else if (cf >= 258 && cf < 258 + 65536) { bits.Put(3, 2); bits.Put(cf - 258, 16); }
+  else return JXL_FAILURE("colour factor out of range");
+  uint32_t hx, hb;
+  if (!HalfBits(p.cfl_base_x, &hx) || !HalfBits(p.cfl_base_b, &hb)) return JXL_FAILURE("base correlation not F16");
+  bits.Put(hx, 16);
+  bits.Put(hb, 16);
+  bits.Put(static_cast<uint32_t>(cc.GetYToXDC() - std::numeric_limits<int8_t>::min()), 8);
+  bits.Put(static_cast<uint32_t>(cc.GetYToBDC() - std::numeric_limits<int8_t>::min()), 8);
+  {
+    BitReader br(Bytes(bits.bytes.data(), bits.bytes.size()));
+    Status st = cmap.DecodeDC(&br);
+    Status closed = br.Close();
+    JXL_RETURN_IF_ERROR(st);
+    JXL_RETURN_IF_ERROR(closed);
+  }
+  if (cmap.base().GetBaseCorrelationX() != p.cfl_base_x || cmap.base().GetBaseCorrelationB() != p.cfl_base_b ||
+      static_cast<uint32_t>(cmap.base().GetColorFactor()) != cf)
+    return JXL_FAILURE("colour correlation not taken");
+
+  if (lf.epf_iters > 0) {   // as the DC groups do after their AC metadata (dec_modular.cc:557-559)
+    const FrameDimensions& d = ds->shared->frame_dim;
+    for (size_t g = 0; g < d.num_dc_groups; g++) JXL_RETURN_IF_ERROR(ComputeSigma(lf, d.DCGroupRect(g), ds));
+  }
+  return true;
+}
+
+}  // namespace
+
+REF_API int ref_frame_set_params(void* h, const RefFrameParams* p) {
+  return SetParamsImpl(static_cast<RefFrame*>(h), *p) ? 0 : 1;
 }
 
 // plane ids for ref_frame_get_plane

@@ -7,7 +7,9 @@ Random frame size (1..700 px), strategy subset, Gaborish/EPF setting, coefficien
 transfer function, stage chain (incl. odd ones -> tile kernel) and hand-off (dense / sparse / shuffled /
 streamed / band by band); every frame is compared bit for bit with the oracle.  End of round 1: 872
 frames over four seeds, no mismatch.  Round 2 adds: EPF engaged on a random subset of the blocks (sharpness 0 / 7,
-quantiser 1: the strip kernel's block permutation), upsampling 2/4/8 with ragged output sizes, noise."""
+quantiser 1: the strip kernel's block permutation), upsampling 2/4/8 with ragged output sizes, noise.  Half of the
+frames carry a random legal non-default frame header (jxl_workload.header_params: Gaborish weights, EPF LUT and
+scales, CfL base, colour factor, quantisation biases, qm scales, opsin matrix and biases, intensity target)."""
 import sys, time, ctypes as C
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parents[2]))
@@ -36,6 +38,9 @@ while time.time() < t_end:
     except Exception as e:
         desc, coeffs = wl.synthetic_frame(w, h, seed=int(rng.integers(1<<30)), gab=gab, epf_iters=epf, ac_type=ac)
     desc.out_format, desc.stage_mask = fmt, srgb
+    hdr = int(rng.integers(1 << 30)) if rng.random() < 0.5 else None
+    if hdr is not None:
+        wl.apply_header(desc, wl.header_params(hdr))
     post = False
     if epf and rng.random() < 0.5:   # EPF really engaged on part of the blocks
         desc.raw_quant = np.where(desc.raw_quant > 0, 1, 0).astype(np.int32)
@@ -55,7 +60,7 @@ while time.time() < t_end:
         if (desc.stage_mask & 14) and epf==0: desc.stage_mask &= ~14
     want = cpu.render_frame(desc, coeffs, rcp_mode=0)
     mode = rng.integers(0,3) if post else rng.integers(0,4)
-    cfg = dict(w=w,h=h,gab=gab,epf=epf,ac=ac,fmt=fmt,mask=hex(desc.stage_mask),mode=int(mode),ups=desc.upsampling,noise=desc.noise)
+    cfg = dict(w=w,h=h,gab=gab,epf=epf,ac=ac,fmt=fmt,mask=hex(desc.stage_mask),mode=int(mode),ups=desc.upsampling,noise=desc.noise,hdr=hdr)
     try:
         if mode==0: got = pipe.decode_frame(desc, coeffs)
         elif mode==1: got = pipe.decode_frame(desc, coeffs, sparse=True, order=rng.permutation(desc.num_groups).tolist(), stream_output=True)
