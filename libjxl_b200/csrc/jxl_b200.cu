@@ -86,7 +86,7 @@ struct jxlgpu_ctx {
   void* host_out = nullptr;
   size_t host_out_stride = 0;
   int stream_error = 0;
-  DevBuf acs, quant, sharp, ytox, ytob, dc, dq, coeff, coeff_off, sigma, list, counts, xyb, out;
+  DevBuf acs, quant, sharp, ytox, ytob, dc, dq, coeff, sigma, list, counts, xyb, out;
   // multi-GPU gather through the copy engines: finished row chunks are copied to the peers' frame buffers on
   // side streams while the next chunk is filtered (JXLGPU_GATHER=kernel keeps the in-kernel replay)
   cudaStream_t rep_streams[8] = {};
@@ -534,7 +534,7 @@ void jxlgpu_destroy(jxlgpu_ctx* ctx) {
   cudaSetDevice(ctx->device);
   cudaDeviceSynchronize();
   for (DevBuf* b : {&ctx->acs, &ctx->quant, &ctx->sharp, &ctx->ytox, &ctx->ytob, &ctx->dc, &ctx->dq,
-                    &ctx->coeff, &ctx->coeff_off, &ctx->sigma,
+                    &ctx->coeff, &ctx->sigma,
                     &ctx->list, &ctx->counts, &ctx->xyb, &ctx->out, &ctx->sparse, &ctx->qdc, &ctx->dc_deq, &ctx->bmap})
     b->release();
   for (auto s : ctx->up_streams)
@@ -635,7 +635,6 @@ int jxlgpu_frame_begin(jxlgpu_ctx* ctx, const jxlgpu_frame* f) {
   CU(ctx->ytob.ensure(cmw * cmh));
   CU(ctx->dc.ensure(3 * nblocks * 4));
   CU(ctx->dq.ensure(f->dequant_table_floats * 4));
-  CU(ctx->coeff_off.ensure(nblocks * 2));
   CU(ctx->sigma.ensure(nblocks * 4));
   CU(ctx->bmap.ensure(nblocks * sizeof(uint4)));
   // per-strategy work lists, capacity = max number of varblocks of that size
@@ -706,7 +705,6 @@ int jxlgpu_frame_begin(jxlgpu_ctx* ctx, const jxlgpu_frame* f) {
     for (int c = 0; c < 3; c++) P.coeff[c] = (uint8_t*)ctx->coeff.p + (size_t)c * 65536 * ctx->elem_size;
     P.coeff_gstride = 3 * 65536;
   }
-  P.coeff_off = (uint16_t*)ctx->coeff_off.p;
   P.sigma = (float*)ctx->sigma.p;
   P.bmap = (uint4*)ctx->bmap.p;
   P.fused = 0;
