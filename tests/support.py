@@ -121,6 +121,132 @@ def header_frame(w: int, h: int, seed: int, hdr, gab: int = 1, epf_iters: int = 
     return desc, coeffs
 
 
+K_MIN_SIGMA = np.float32(-3.90524291751269967465540850526868)   # epf.h: blocks with 1/sigma below it skip the EPF
+EPF_STAGES = abi.STAGE_EPF0 | abi.STAGE_EPF1 | abi.STAGE_EPF2
+
+
+def block_quant(desc: abi.FrameDesc) -> np.ndarray:
+    """raw_quant of the varblock covering each 8x8 block (raw_quant itself is defined on first blocks only)."""
+    acs = desc.ac_strategy
+    out = np.zeros(acs.shape, np.int64)
+    first = (acs & 1) == 1
+    for s in range(27):
+        ys, xs = np.nonzero(first & ((acs >> 1) == s))
+        for iy in range(abi.COVERED_Y[s]):
+            for ix in range(abi.COVERED_X[s]):
+                out[ys + iy, xs + ix] = desc.raw_quant[ys, xs]
+    return out
+
+
+def epf_frame(w: int, h: int, seed: int, gab: int = 1, epf_iters: int = 3, ac_type: int = abi.AC_INT16, hdr=None,
+              strategies: str = "all"):
+    """A synthetic frame on which the EPF does real work everywhere: about half of the varblocks get a quantiser
+    1..4, the rest 40..256 (EPF skipped), every block a sharpness 0..7, so engaged and skipped blocks mix inside
+    every block row of every 256-column strip (the strip kernel's block permutation is not the identity).  Varblocks
+    32 or more columns wide always get a quantiser 1..2, else one large transform of high quantiser would leave a
+    whole strip block row unfiltered.  Small, clipped coefficients keep the SADs small enough that many EPF weights lie
+    strictly inside (0, 1).  `hdr`: a jxl_workload.header_params name or seed."""
+    desc, coeffs = wl.synthetic_frame(w, h, seed=seed, strategies=strategies, gab=gab, epf_iters=epf_iters,
+                                      ac_type=ac_type, density=0.08)
+    rng = np.random.default_rng(seed + 4242)
+    shape = desc.raw_quant.shape
+    acs = desc.ac_strategy
+    wide = np.array([abi.COVERED_X[s] >= 4 for s in range(27)])[acs >> 1]
+    q = np.where(rng.random(shape) < 0.5, rng.integers(1, 5, shape), rng.integers(40, 257, shape))
+    q = np.where(wide, rng.integers(1, 3, shape), q)
+    desc.raw_quant = np.where((acs & 1) == 1, q, 0).astype(np.int32)
+    desc.epf_sharpness = rng.integers(0, 8, shape).astype(np.uint8)
+    coeffs = np.clip(coeffs, -3, 3)
+    # a flat block is a fixed point of the EPF and a block edge of synthetic_frame's DC noise zeroes every weight
+    # across it: a tenth of the DC noise and 1/25 of the AC amplitude leave SADs where the weights are neither
+    mean = desc.dc.mean(axis=(1, 2), keepdims=True)
+    desc.dc = (mean + np.float32(0.1) * (desc.dc - mean)).astype(np.float32)
+    desc.dequant = (desc.dequant * np.float32(0.04)).astype(np.float32)
+    if hdr is not None:
+        wl.apply_header(desc, wl.header_params(hdr))
+    eng = epf_engaged_blocks(desc)
+    frac = eng.mean()
+    assert 0.2 <= frac <= 0.75, frac
+    # every block row of every full 32-block strip holds engaged and skipped blocks
+    xb = desc.xsize_blocks
+    for x0 in range(0, xb - 31, 32):
+        part = eng[:, x0:x0 + 32]
+        assert part.any(1).all() and (~part).any(1).all(), (w, h, seed, x0)
+    return desc, coeffs
+
+
+def epf_engaged_blocks(desc: abi.FrameDesc) -> np.ndarray:
+    """(ysize_blocks, xsize_blocks) bool: blocks whose inverse sigma (the oracle's ComputeSigma) engages the EPF."""
+    from oracle import cpu as ocpu
+    return ~(ocpu.compute_sigma(desc)[2:-2, 2:-2] < K_MIN_SIGMA)
+
+
+def without_epf(desc: abi.FrameDesc) -> abi.FrameDesc:
+    """The same stage chain with every EPF pass taken out."""
+    import dataclasses
+    if desc.stage_mask & abi.STAGE_EXPLICIT:
+        return dataclasses.replace(desc, stage_mask=desc.stage_mask & ~EPF_STAGES)
+    return dataclasses.replace(desc, epf_iters=0)
+
+
+def changed_pixels(a: np.ndarray, b: np.ndarray, planar: bool) -> np.ndarray:
+    """(H, W) bool: pixels where any channel of two renders differs."""
+    d = a != b
+    return d.any(0) if planar else d.reshape(d.shape[0], d.shape[1], -1).any(2)
+
+
+def epf_coverage(desc: abi.FrameDesc, coeffs: np.ndarray, render=None, with_epf: np.ndarray | None = None) -> np.ndarray:
+    """The oracle's changed-pixel mask of the EPF: the frame's chain against the same chain without EPF passes.
+    `render(desc)` renders through the oracle (a caching one, say); `with_epf`: the chain's image if at hand."""
+    if render is None:
+        from oracle import cpu as ocpu
+        render = lambda d: ocpu.render_frame(d, coeffs, rcp_mode=0)   # noqa: E731
+    a = with_epf if with_epf is not None else render(desc)
+    return changed_pixels(a, render(without_epf(desc)), desc.out_format == abi.OUT_PLANAR_F32)
+
+
+def _every_window(any_: np.ndarray, n: int) -> bool:
+    """True if every window of n consecutive entries (the whole array if shorter) holds a True."""
+    if any_.size <= n:
+        return bool(any_.any())
+    c = np.concatenate([[0], np.cumsum(any_)])
+    return bool((c[n:] - c[:-n] > 0).all())
+
+
+def assert_epf_coverage(mask: np.ndarray, what: str, boundary_min: int = 200, band_rows=None) -> None:
+    """Every group-row boundary (and the `band_rows` boundaries) +-7 rows holds at least `boundary_min` changed
+    pixels; every 64-row window (the strip kernel's shortest row segment) and every 240-column window (a fused-kernel
+    strip) holds one.  Prints the figures."""
+    h, w = mask.shape
+    bounds = sorted(set(range(abi.GROUP_DIM, h, abi.GROUP_DIM)) | set(band_rows or ()))
+    counts = [int(mask[max(0, y - 7):y + 7].sum()) for y in bounds]
+    rows, cols = mask.any(1), mask.any(0)
+    print(f"EPF coverage {what}: {mask.mean():.2%} of pixels changed; +-7 rows around {len(bounds)} boundaries: "
+          f"min {min(counts, default=0)} changed; 64-row windows all hit: {_every_window(rows, 64)}; "
+          f"240-column windows all hit: {_every_window(cols, 240)}")
+    assert all(c >= boundary_min for c in counts), (what, list(zip(bounds, counts)))
+    assert _every_window(rows, 64), what
+    assert _every_window(cols, 240), what
+
+
+def decoy_frame(desc: abi.FrameDesc, seed: int):
+    """A frame of the same geometry, ac_type, chain and output as `desc` with other coefficients, a DC offset and
+    the EPF engaged on every block.  Rendered on a context just before `desc`, it leaves every device buffer full of
+    values that are wrong for `desc`: a kernel that reads a row before it is written shows it in the pixels."""
+    import dataclasses
+    d, coeffs = wl.synthetic_frame(desc.xsize, desc.ysize, seed=seed, gab=desc.gab, epf_iters=3, ac_type=desc.ac_type,
+                                   density=0.05)
+    d = dataclasses.replace(desc, ac_strategy=d.ac_strategy, dc=d.dc + np.float32(0.05), ytox=d.ytox, ytob=d.ytob,
+                            raw_quant=np.where(d.raw_quant > 0, 1, 0).astype(np.int32),
+                            epf_sharpness=np.full_like(d.epf_sharpness, 7))
+    return d, np.clip(coeffs, -2, 2)
+
+
+def assert_decoy_differs(decoy_px: np.ndarray, want: np.ndarray, planar: bool, min_frac: float = 0.99) -> None:
+    frac = changed_pixels(decoy_px, want, planar).mean()
+    assert frac >= min_frac, f"the decoy matches the target on {1 - frac:.2%} of the pixels"
+
+
 def dc_stage_input(xs: int, ys: int) -> np.ndarray:
     """Seeded quantised DC planes (X, Y, B): smooth gradients (adaptive smoothing engages) with one busy
     quadrant (it must switch itself off there)."""
