@@ -283,8 +283,10 @@ JXLGPU_API int jxlgpu_render_device(jxlgpu_ctx* ctx, void* dev_out, size_t out_s
 JXLGPU_API int jxlgpu_set_output_replicas(jxlgpu_ctx* ctx, uint32_t n, void* const* dev_ptrs, void* multicast_ptr);
 /* Context-owned output buffer of the last render (device pointer) and its row stride. */
 JXLGPU_API int jxlgpu_device_output(jxlgpu_ctx* ctx, void** dev_ptr, size_t* stride_bytes);
-/* Post-IDCT XYB planes [3][ysize_blocks*8][xsize_blocks*8] (device pointer): halo exchange
- * between bands and stage taps. */
+/* Post-IDCT XYB planes [3][ysize_blocks*8][xsize_blocks*8], row-major (device pointer): halo
+ * exchange between bands and stage taps.  The renders keep this intermediate in 8x8 block tiles; the
+ * call synchronises with the last render, copies it into a context-owned row-major buffer (one
+ * kernel launch) and returns that buffer, valid until the next call, frame_begin or destroy. */
 JXLGPU_API int jxlgpu_device_xyb(jxlgpu_ctx* ctx, float** dev_ptr, size_t* plane_stride_floats,
                                  size_t* row_stride_floats);
 JXLGPU_API int jxlgpu_synchronize(jxlgpu_ctx* ctx);

@@ -87,6 +87,7 @@ struct jxlgpu_ctx {
   size_t host_out_stride = 0;
   int stream_error = 0;
   DevBuf acs, quant, sharp, ytox, ytob, dc, dq, coeff, sigma, list, counts, xyb, out;
+  DevBuf xyb_rows;            // jxlgpu_device_xyb: row-major copy of the (block-tiled) XYB intermediate
   // multi-GPU gather through the copy engines: finished row chunks are copied to the peers' frame buffers on
   // side streams while the next chunk is filtered (JXLGPU_GATHER=kernel keeps the in-kernel replay)
   cudaStream_t rep_streams[8] = {};
@@ -535,7 +536,7 @@ void jxlgpu_destroy(jxlgpu_ctx* ctx) {
   cudaDeviceSynchronize();
   for (DevBuf* b : {&ctx->acs, &ctx->quant, &ctx->sharp, &ctx->ytox, &ctx->ytob, &ctx->dc, &ctx->dq,
                     &ctx->coeff, &ctx->sigma,
-                    &ctx->list, &ctx->counts, &ctx->xyb, &ctx->out, &ctx->sparse, &ctx->qdc, &ctx->dc_deq, &ctx->bmap})
+                    &ctx->list, &ctx->counts, &ctx->xyb, &ctx->xyb_rows, &ctx->out, &ctx->sparse, &ctx->qdc, &ctx->dc_deq, &ctx->bmap})
     b->release();
   for (auto s : ctx->up_streams)
     if (s) cudaStreamDestroy(s);
@@ -644,8 +645,7 @@ int jxlgpu_frame_begin(jxlgpu_ctx* ctx, const jxlgpu_frame* f) {
     total += nblocks / (covered_x(s) * covered_y(s)) + 1;
   }
   CU(ctx->list.ensure(total * sizeof(uint4)));
-  P.row_stride = xb * 8;
-  P.plane_stride = P.row_stride * yb * 8;
+  P.plane_stride = (size_t)xb * yb * 64;   // [3][yb][xb][64]: 8x8 block tiles (FrameDev::xyb_off)
   CU(ctx->xyb.ensure(3 * P.plane_stride * 4));
   // host-fed coefficients live group-major on the device: [group][channel][65536]
   if (!ctx->coeff_external) CU(ctx->coeff.ensure((size_t)ctx->num_groups * 3 * 65536 * ctx->elem_size));
@@ -1198,10 +1198,24 @@ int jxlgpu_device_output(jxlgpu_ctx* ctx, void** dev_ptr, size_t* stride_bytes) 
 
 int jxlgpu_device_xyb(jxlgpu_ctx* ctx, float** dev_ptr, size_t* plane_stride_floats, size_t* row_stride_floats) {
   if (!ctx || !dev_ptr) return JXLGPU_ERR_INVALID_ARGUMENT;
-  *dev_ptr = (float*)ctx->xyb.p;
-  if (plane_stride_floats) *plane_stride_floats = ctx->P.plane_stride;
-  if (row_stride_floats) *row_stride_floats = ctx->P.row_stride;
-  return ctx->xyb.p ? JXLGPU_OK : JXLGPU_ERR_STATE;
+  if (!ctx->xyb.p) return JXLGPU_ERR_STATE;
+  CU(cudaSetDevice(ctx->device));
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  // the renders keep the intermediate in 8x8 block tiles: hand out a row-major copy, made after the last
+  // render (which may have run on the caller's stream) and complete on return
+  const FrameDev& P = ctx->P;
+  CU(ctx->xyb_rows.ensure(3 * P.plane_stride * sizeof(float)));
+  if (ctx->ext_pending) CU(cudaStreamWaitEvent(ctx->stream, ctx->ev_ext_done, 0));
+  const size_t n4 = 3 * P.plane_stride / 4;
+  const unsigned grid = (unsigned)std::min<size_t>((n4 + 255) / 256, (size_t)ctx->num_sms * 8);
+  xyb_untile_kernel<<<grid, 256, 0, ctx->stream>>>(P, (float*)ctx->xyb_rows.p);
+  CU(cudaGetLastError());
+  ctx->launches += 1;
+  CU(cudaStreamSynchronize(ctx->stream));
+  *dev_ptr = (float*)ctx->xyb_rows.p;
+  if (plane_stride_floats) *plane_stride_floats = P.plane_stride;
+  if (row_stride_floats) *row_stride_floats = (size_t)P.xb * 8;
+  return JXLGPU_OK;
 }
 
 int jxlgpu_synchronize(jxlgpu_ctx* ctx) {

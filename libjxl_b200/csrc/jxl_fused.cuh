@@ -691,7 +691,7 @@ fused_tile_kernel(const __grid_constant__ FrameDev P, char* __restrict__ out, si
             if (kc == (int)kBmapSkip) continue;
             if (kc == (int)kBmapCopy) {
               if (act) {  // lane l copies pixel row l of the block from the XYB planes
-                const float* src = P.xyb + ((size_t)B * 8 + l) * P.row_stride + (size_t)(bx0 + bxl) * 8;
+                const float* src = P.xyb_block(0, B, bx0 + bxl) + l * 8;
 #pragma unroll
                 for (int c = 0; c < 3; c++) {
                   const float4 a = __ldg(reinterpret_cast<const float4*>(src + (size_t)c * P.plane_stride));

@@ -119,9 +119,23 @@ struct FrameDev {
   // and no work lists for the 8x8 class (the fused kernel transforms those itself).
   uint4* bmap;
   uint32_t fused;
-  // planes
-  float* xyb;                // 3 planes [yb*8][xb*8]
-  size_t plane_stride, row_stride;
+  // the XYB intermediate (inverse transforms -> filters): per channel, the 8x8 blocks in raster order, each
+  // block 64 contiguous floats in row-major order ([3][yb][xb][64]).  One block of one channel is two whole
+  // 128-byte lines, so the 8x8 transform writes full lines.  Every kernel addresses it through xyb_off /
+  // xyb_at / xyb_block below.
+  float* xyb;
+  size_t plane_stride;       // floats per channel: xb * yb * 64
+  // offset of pixel (y, x) from pixel (0, 0) of a channel; additive in y and x (xyb_off(y, x) ==
+  // xyb_off(y, 0) + xyb_off(0, x)), so it also gives offsets relative to any block corner
+  __host__ __device__ __forceinline__ size_t xyb_off(int y, int x) const {
+    return ((size_t)(y >> 3) * xb + (x >> 3)) * 64 + (y & 7) * 8 + (x & 7);
+  }
+  __host__ __device__ __forceinline__ float* xyb_at(int c, int y, int x) const {
+    return xyb + (size_t)c * plane_stride + xyb_off(y, x);
+  }
+  __host__ __device__ __forceinline__ float* xyb_block(int c, int by, int bx) const {
+    return xyb + (size_t)c * plane_stride + ((size_t)by * xb + bx) * 64;
+  }
   // scalars
   float inv_global_scale, quant_scale, x_dm, b_dm;
   float qbias[4];
@@ -247,6 +261,18 @@ __device__ __forceinline__ void st_global_l2_keep(float* p, float4 v) {
                "f"(v.w), "l"(pol) : "memory");
 #else
   *reinterpret_cast<float4*>(p) = v;
+#endif
+}
+// Read-only load of one float of the XYB intermediate with a 256-byte L2 prefetch size (ld.global.nc.L2::256B):
+// an L2 miss brings the whole 8x8 block of that channel from HBM, the seven rows the strip filter reads from it
+// in the next steps included, instead of one 32-byte sector per row.
+__device__ __forceinline__ float ldg_xyb(const float* p) {
+#if JXLB_PTX
+  float v;
+  asm("ld.global.nc.L2::256B.f32 %0, [%1];" : "=f"(v) : "l"(p));
+  return v;
+#else
+  return __ldg(p);
 #endif
 }
 // generic-proxy writes to shared memory -> visible to the async proxy (the TMA unit)
@@ -573,9 +599,9 @@ __device__ __forceinline__ void small_dct_item(const FrameDev& P, int kind, uint
 #pragma unroll
       for (int j = 0; j < R; j++) u[j] = T[j * (C + 1) + l];
       idct1d<R>(u);
-      float* out = P.xyb + (size_t)c * P.plane_stride + (size_t)vb.aby * 8 * P.row_stride + vb.abx * 8 + l;
+      float* out = P.xyb_at(c, vb.aby * 8, vb.abx * 8 + l);
 #pragma unroll
-      for (int y = 0; y < R; y++) out[(size_t)y * P.row_stride] = u[y];
+      for (int y = 0; y < R; y++) out[P.xyb_off(y, 0)] = u[y];
     }
     __syncwarp();
   }
@@ -730,8 +756,10 @@ __device__ __forceinline__ void block8_dequant(const FrameDev& P, int dqkind, co
 }
 
 // Where the pixels of an 8x8-class block go.
-//   Block8ToPlanes: the XYB planes in HBM (idct8_kernel).  The specials assemble the block in a 64-float
-//     scratch (row pitch 8) and lane l stores pixel row l with two 16-byte stores.
+//   Block8ToPlanes: the XYB intermediate in HBM (idct8_kernel), where a block of one channel is 256
+//     contiguous bytes (FrameDev::xyb_block).  The block is assembled in a 64-float scratch (row pitch 8,
+//     i.e. the block's own layout) and the slot's 8 lanes store it as two whole 128-byte lines: lane l
+//     writes floats 4l .. 4l+3 and 32+4l .. 35+4l.
 //   (the fused kernel's policy, Block8ToRing in jxl_fused.cuh, writes straight into its shared-memory
 //     pixel ring: row pitch = one ring row.)
 // Interface: kPitch; px(c) = where pixel (y, x) of channel c is assembled (px(c)[y * kPitch + x]);
@@ -743,30 +771,23 @@ struct Block8ToPlanes {
   static constexpr bool kGuardPx = false;  // inactive slots assemble garbage in their own scratch
   static constexpr bool kDctRows = true;
   float* scratch;
-  float* plane0;  // channel 0, pixel (0, 0) of the block
-  size_t plane_stride, row_stride;
+  float* block0;  // channel 0 of the block (P.xyb_block(0, by, bx))
+  size_t plane_stride;
   __device__ __forceinline__ float* px(int) const { return scratch; }
-  // lane l stores the half (l & 1) of rows (l >> 1) and (l >> 1) + 4: each 16-byte store instruction of a warp
-  // writes four whole 32-byte rows per block (column stores take eight instructions per channel)
-  __device__ __forceinline__ void dct_rows(int c, int l, const float* px, bool active) const {
-    if (active) {
+  // each 16-byte store instruction of a warp writes one whole 128-byte line per block
+  __device__ __forceinline__ void store_block(int c, int l, const float* px) const {
 #pragma unroll
-      for (int k = 0; k < 2; k++) {
-        const int y = (l >> 1) + 4 * k, h = (l & 1) * 4;
-        const float4 a = *reinterpret_cast<const float4*>(px + y * 8 + h);
-        st_global_l2_keep(plane0 + (size_t)c * plane_stride + (size_t)y * row_stride + h, a);
-      }
+    for (int k = 0; k < 2; k++) {
+      const float4 a = *reinterpret_cast<const float4*>(px + 32 * k + 4 * l);
+      st_global_l2_keep(block0 + (size_t)c * plane_stride + 32 * k + 4 * l, a);
     }
+  }
+  __device__ __forceinline__ void dct_rows(int c, int l, const float* px, bool active) const {
+    if (active) store_block(c, l, px);
   }
   __device__ __forceinline__ void finish(int c, int l, bool active) const {
     __syncwarp();
-    if (active) {  // lane l stores pixel row l (2 x 16 B)
-      float* out = plane0 + (size_t)c * plane_stride + (size_t)l * row_stride;
-      const float4 a = *reinterpret_cast<const float4*>(scratch + l * 8);
-      const float4 b = *reinterpret_cast<const float4*>(scratch + l * 8 + 4);
-      st_global_l2_keep(out, a);
-      st_global_l2_keep(out + 4, b);
-    }
+    if (active) store_block(c, l, scratch);
     __syncwarp();
   }
 };
@@ -815,7 +836,7 @@ __device__ __forceinline__ void block8_transform(int kind, bool active, const fl
     }
     __syncwarp();
     if constexpr (Out::kDctRows) {
-#pragma unroll
+#pragma unroll 1  // (unrolled, idct8_tma_kernel<false> spills 12 bytes at its 64-register limit)
       for (int c = 0; c < 3; c++) out.dct_rows(c, l, scr + c * 64, active);
       __syncwarp();
     }
@@ -1100,9 +1121,8 @@ __device__ __forceinline__ void block8_item(const FrameDev& P, int kind, uint4 e
   }
   Block8ToPlanes out;
   out.scratch = scr + 192;
-  out.plane0 = P.xyb + (size_t)vb.aby * 8 * P.row_stride + vb.abx * 8;
+  out.block0 = P.xyb_block(0, vb.aby, vb.abx);
   out.plane_stride = P.plane_stride;
-  out.row_stride = P.row_stride;
   block8_transform(kind, active, val, l, scr, out);
 }
 
@@ -1313,9 +1333,8 @@ __global__ void __launch_bounds__(kTma8Warps * 32, 2) idct8_tma_kernel(const __g
     __syncwarp();  // every lane holds its coefficients: the staging words become the transform's scratch
     Block8ToPlanes out;
     out.scratch = scr + 128;
-    out.plane0 = P.xyb + (size_t)vb.aby * 8 * P.row_stride + vb.abx * 8;
+    out.block0 = P.xyb_block(0, vb.aby, vb.abx);
     out.plane_stride = P.plane_stride;
-    out.row_stride = P.row_stride;
     block8_transform(kind, act_cur, val, l, scr, out);
     // buffer `st` is free: the item after next goes there (its record, fetched last iteration, has landed)
     fence_async_smem();
@@ -1473,10 +1492,10 @@ __device__ __forceinline__ void large_item(const FrameDev& P, int kind, uint4 en
           for (int k = 0; k < CX; k++) v[k] = llf[c * CY * CX + j * CX + k];
         }
         idct1d<C>(v);
-        float* out = P.xyb + (size_t)c * P.plane_stride + ((size_t)vb.aby * 8 + j) * P.row_stride + vb.abx * 8;
+        float* out = P.xyb_at(c, vb.aby * 8 + j, vb.abx * 8);
 #pragma unroll
         for (int x = 0; x < C; x += 4)
-          *reinterpret_cast<float4*>(out + x) = make_float4(v[x], v[x + 1], v[x + 2], v[x + 3]);
+          *reinterpret_cast<float4*>(out + P.xyb_off(0, x)) = make_float4(v[x], v[x + 1], v[x + 2], v[x + 3]);
       }
     } else {
       constexpr int NB = 1024 / C;                 // rows per warp
@@ -1498,8 +1517,8 @@ __device__ __forceinline__ void large_item(const FrameDev& P, int kind, uint4 en
       __syncwarp();
       idct1d_warp<C, 1024>(buf, buf + 1024);
       for (int b = 0; b < NB; b++) {
-        float* out = P.xyb + (size_t)c * P.plane_stride + ((size_t)vb.aby * 8 + jw + b) * P.row_stride + vb.abx * 8;
-        for (int x = lane; x < C; x += 32) out[x] = buf[b * C + x];
+        float* out = P.xyb_at(c, vb.aby * 8 + jw + b, vb.abx * 8);
+        for (int x = lane; x < C; x += 32) out[P.xyb_off(0, x)] = buf[b * C + x];
       }
       __syncwarp();
     }
@@ -1509,22 +1528,22 @@ __device__ __forceinline__ void large_item(const FrameDev& P, int kind, uint4 en
       const int r = slab * 256 + tid;
       if (r < 3 * C) {
         const int c = r / C, x = r % C;
-        float* col = P.xyb + (size_t)c * P.plane_stride + (size_t)vb.aby * 8 * P.row_stride + vb.abx * 8 + x;
+        float* col = P.xyb_at(c, vb.aby * 8, vb.abx * 8 + x);
         float u[R];
 #pragma unroll
-        for (int j = 0; j < R; j++) u[j] = col[(size_t)j * P.row_stride];
+        for (int j = 0; j < R; j++) u[j] = col[P.xyb_off(j, 0)];
         idct1d<R>(u);
 #pragma unroll
-        for (int y = 0; y < R; y++) col[(size_t)y * P.row_stride] = u[y];
+        for (int y = 0; y < R; y++) col[P.xyb_off(y, 0)] = u[y];
       }
     } else {
-      // 32 columns of one channel: the [R][32] tile travels between the plane and shared memory in
-      // full 128-byte rows; each warp transforms 4 of its columns at a time
+      // 32 columns (four blocks) of one channel: the [R][32] tile travels between the plane and shared memory
+      // a row at a time (four 32-byte block rows); each warp transforms 4 of its columns at a time
       constexpr int XS = C / 32;  // column slabs per channel
       const int c = slab / XS, x0 = (slab % XS) * 32;
       float* tile = sm + kLargeTileOff;  // [R][33]
-      float* base = P.xyb + (size_t)c * P.plane_stride + (size_t)vb.aby * 8 * P.row_stride + vb.abx * 8 + x0;
-      for (int j = warp; j < R; j += kLargeWarps) tile[j * 33 + lane] = base[(size_t)j * P.row_stride + lane];
+      float* base = P.xyb_at(c, vb.aby * 8, vb.abx * 8 + x0);
+      for (int j = warp; j < R; j += kLargeWarps) tile[j * 33 + lane] = base[P.xyb_off(j, lane)];
       __syncthreads();
       float* buf = coop + warp * 2048;
       for (int e = lane; e < 4 * R; e += 32) buf[e] = tile[(e % R) * 33 + 4 * warp + e / R];
@@ -1532,7 +1551,7 @@ __device__ __forceinline__ void large_item(const FrameDev& P, int kind, uint4 en
       idct1d_warp<R, 4 * R>(buf, buf + 1024);
       for (int e = lane; e < 4 * R; e += 32) tile[(e % R) * 33 + 4 * warp + e / R] = buf[e];
       __syncthreads();
-      for (int j = warp; j < R; j += kLargeWarps) base[(size_t)j * P.row_stride + lane] = tile[j * 33 + lane];
+      for (int j = warp; j < R; j += kLargeWarps) base[P.xyb_off(j, lane)] = tile[j * 33 + lane];
     }
   }
   __syncthreads();
@@ -2125,6 +2144,17 @@ __global__ void __launch_bounds__(256) upsample_in_kernel(const __grid_constant_
   }
 }
 
+// jxlgpu_device_xyb: the block-tiled XYB intermediate as row-major planes [3][yb*8][xb*8] (same size and plane
+// stride), one float4 (half a block row) per thread and step
+__global__ void __launch_bounds__(256) xyb_untile_kernel(const __grid_constant__ FrameDev P, float* __restrict__ out) {
+  const size_t W = (size_t)P.xb * 8, n4 = 3 * P.plane_stride / 4;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t e = 4 * i, r = e % P.plane_stride;
+    const int c = (int)(e / P.plane_stride), y = (int)(r / W), x = (int)(r % W);
+    *reinterpret_cast<float4*>(out + e) = *reinterpret_cast<const float4*>(P.xyb_at(c, y, x));
+  }
+}
+
 __global__ void __launch_bounds__(kFilterThreads) filter_kernel(const __grid_constant__ FrameDev P,
                                                                char* __restrict__ out,
                                                                size_t out_row_stride /*bytes*/) {
@@ -2150,7 +2180,7 @@ __global__ void __launch_bounds__(kFilterThreads) filter_kernel(const __grid_con
     for (int i = tid; i < SH * SW; i += kFilterThreads) {
       const int ty = i / SW, tx = i % SW;
       const int y = G.y0 + ty, x = G.x0 + tx;
-      if (y >= 0 && y < H && x >= 0 && x < W) bufA[c * kTilePlane + ty * kSP + tx] = src[(size_t)y * P.row_stride + x];
+      if (y >= 0 && y < H && x >= 0 && x < W) bufA[c * kTilePlane + ty * kSP + tx] = src[P.xyb_off(y, x)];
     }
   }
   __syncthreads();
@@ -2483,13 +2513,15 @@ __device__ __forceinline__ void filter_strip_body(const FrameDev& P, char* __res
   const int r_end = hi(0) + d2;  // after this many input-row steps the last output row is out
   const float kMinSigma = -3.90524291751269967465540850526868f;
 
-  // row r_in_lo is fetched up front, every later row one step ahead of its use
+  // row r_in_lo is fetched up front, every later row one step ahead of its use.  A warp's 32 columns of a row
+  // are four 32-byte block rows (FrameDev::xyb_off)
+  const size_t xoff = xin ? P.xyb_off(0, x) : 0;
   float pre_a = 0.0f, pre_b = 0.0f, pre_c = 0.0f;
   if (r_in_lo < r_in_hi && xin) {
-    const size_t off = (size_t)r_in_lo * P.row_stride + x;
-    pre_a = __ldg(P.xyb + off);
-    pre_b = __ldg(P.xyb + P.plane_stride + off);
-    pre_c = __ldg(P.xyb + 2 * P.plane_stride + off);
+    const size_t off = P.xyb_off(r_in_lo, 0) + xoff;
+    pre_a = ldg_xyb(P.xyb + off);
+    pre_b = ldg_xyb(P.xyb + P.plane_stride + off);
+    pre_c = ldg_xyb(P.xyb + 2 * P.plane_stride + off);
   }
 
   // inverse sigma of each EPF stage's next row, fetched one step ahead as well.  A stage's first
@@ -2595,10 +2627,10 @@ __device__ __forceinline__ void filter_strip_body(const FrameDev& P, char* __res
       if ((J >= 0 ? J == 7 : ((rin + 1) & 7) == 0) && rin + 1 < r_in_hi) build_lists(rin + 1);
     }
     if (rin + 1 < r_in_hi && xin) {
-      const size_t off = (size_t)(rin + 1) * P.row_stride + x;
-      pre_a = __ldg(P.xyb + off);
-      pre_b = __ldg(P.xyb + P.plane_stride + off);
-      pre_c = __ldg(P.xyb + 2 * P.plane_stride + off);
+      const size_t off = P.xyb_off(rin + 1, 0) + xoff;
+      pre_a = ldg_xyb(P.xyb + off);
+      pre_b = ldg_xyb(P.xyb + P.plane_stride + off);
+      pre_c = ldg_xyb(P.xyb + 2 * P.plane_stride + off);
     }
     // ---- Gaborish (stage_gaborish.cc:56-100) ----
     if constexpr (C::G) {
