@@ -279,7 +279,9 @@ JXLGPU_API int jxlgpu_render_device(jxlgpu_ctx* ctx, void* dev_out, size_t out_s
  * the filtering and no collective kernel runs.  If multicast_ptr is non-NULL it is the slot's NVSwitch
  * multicast address and one multimem.st.v2 per 8 bytes replaces the n stores.  n = 0 and NULL switch it
  * off.  The caller owns the cross-GPU barrier that publishes the frame (bench.py: symmetric-memory
- * barrier).  Only the production stage chains (filter_strip_kernel) replicate. */
+ * barrier).  Only the production stage chains (filter_strip_kernel) replicate.  Frames with upsampling or
+ * noise do not replicate: jxlgpu_render_device returns JXLGPU_ERR_UNSUPPORTED for them while replicas or a
+ * multicast address are set, before enqueuing anything (as frame_begin refuses them in bands). */
 JXLGPU_API int jxlgpu_set_output_replicas(jxlgpu_ctx* ctx, uint32_t n, void* const* dev_ptrs, void* multicast_ptr);
 /* Context-owned output buffer of the last render (device pointer) and its row stride. */
 JXLGPU_API int jxlgpu_device_output(jxlgpu_ctx* ctx, void** dev_ptr, size_t* stride_bytes);

@@ -308,7 +308,7 @@ int launch_filter(jxlgpu_ctx* ctx, uint32_t y0, uint32_t y1, uint32_t out_y0, ui
     // the filters run at the coded size into planar XYB; upsample_kernel (launch_upsample) carries the
     // stages behind the upsampling: XYB -> RGB, transfer function, packing
     // (the production chains keep their strip-kernel instantiation: the XYB bit stays in the mask, the kernel
-    //  skips the conversion at run time; other masks fall to the generic tile kernel without the bit)
+    //  skips the conversion at run time; other chains run the generic tile kernel without the bit)
     const bool strip_chain = !ctx->force_generic_filter && (P.stage_mask & 16u);
     P.skip_xyb = strip_chain ? 1u : 0u;
     P.stage_mask &= strip_chain ? 31u : 15u;
@@ -329,7 +329,12 @@ int launch_filter(jxlgpu_ctx* ctx, uint32_t y0, uint32_t y1, uint32_t out_y0, ui
     P.fused = 1u | (aligned ? 2u : 0u);
     strip_err = launch_fused(ctx, P, dev_out, out_row_stride, s);
   } else if (!launch_strip(ctx, P, dev_out, out_row_stride, s, &strip_err)) {
-    // stage chains outside the production set (test taps): generic tile kernel
+    // stage chains outside the production set (test taps): generic tile kernel.  It has no skip_xyb: in front
+    // of the upsampling its mask must stop before XYB -> RGB (an explicit chain keeps the bit up to here)
+    if (P.skip_xyb) {
+      P.stage_mask &= 15u;
+      P.skip_xyb = 0;
+    }
     dim3 grid((P.xsize + kTW - 1) / kTW, (y1 - y0 + kTH - 1) / kTH);
     filter_kernel<<<grid, kFilterThreads, kFilterSmemFloats * sizeof(float), s>>>(P, dev_out, out_row_stride);
   }
@@ -1060,6 +1065,8 @@ static int render_device_on(jxlgpu_ctx* ctx, void* dev_out, size_t out_stride_by
     // bases 8-byte aligned), and the multicast mapping moves 4-byte granules (f32 layouts only)
     if ((uintptr_t)o % 8) return JXLGPU_ERR_INVALID_ARGUMENT;
     if (P.mc && P.out_format > JXLGPU_OUT_PLANAR_F32) return JXLGPU_ERR_UNSUPPORTED;
+    // upsampled / noisy frames are finished by upsample_kernel, which writes the local buffer only
+    if (P.ups || P.noise) return JXLGPU_ERR_UNSUPPORTED;
   }
   int rc = launch_idct(ctx, ctx->need_row0, ctx->need_row1, P.need_y0, P.need_y1, s);
   if (rc) return rc;

@@ -44,6 +44,8 @@ def lib():
         L.jxo_make_unsigned.argtypes = [C.c_float, C.c_int, C.c_size_t, C.c_size_t, C.c_int]
         L.jxo_f16_from_f32.restype = C.c_uint16
         L.jxo_f16_from_f32.argtypes = [C.c_float]
+        L.jxo_noise_planes.restype = None
+        L.jxo_noise_planes.argtypes = [C.c_uint32, C.c_uint32, C.c_size_t, C.c_size_t, C.c_void_p]
         _lib = L
     return _lib
 
@@ -98,6 +100,13 @@ def render_frame(desc: abi.FrameDesc, coeffs: np.ndarray, rcp_mode: int = 0) -> 
     rc = lib().jxo_render_frame(C.byref(s), ptrs, rcp_mode, out.ctypes.data)
     if rc:
         raise RuntimeError(f"jxo_render_frame rc={rc}")
+    return out
+
+
+def noise_planes(visible: int, nonvisible: int, w: int, h: int) -> np.ndarray:
+    """Random3Planes before the convolution: (3, h, w) float32 in [1, 2), one generator per 256x256 output tile."""
+    out = np.zeros((3, h, w), np.float32)
+    lib().jxo_noise_planes(visible, nonvisible, w, h, out.ctypes.data)
     return out
 
 

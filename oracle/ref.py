@@ -90,6 +90,12 @@ def can_set_params() -> bool:
     return hasattr(lib(), "ref_frame_set_params")
 
 
+def can_set_ups_noise() -> bool:
+    """Whether the selected harness build has ref_frame_set_upsampling_weights and ref_frame_set_noise_lut
+    (Frame.set_upsampling_weights / set_noise_lut); an older prebuilt oracle/_ref does not."""
+    return hasattr(lib(), "ref_frame_set_upsampling_weights") and hasattr(lib(), "ref_frame_set_noise_lut")
+
+
 def use_variant(variant: str) -> None:
     """'default' = the reference's own build flags; 'strict' = + -ffp-contract=off."""
     global _variant
@@ -114,6 +120,10 @@ def lib():
         L.ref_frame_info.argtypes = [C.c_void_p, C.POINTER(RefFrameInfo)]
         if hasattr(L, "ref_frame_set_params"):   # (absent from a harness built before it existed)
             L.ref_frame_set_params.argtypes = [C.c_void_p, C.POINTER(RefFrameParams)]
+        if hasattr(L, "ref_frame_set_upsampling_weights"):
+            L.ref_frame_set_upsampling_weights.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        if hasattr(L, "ref_frame_set_noise_lut"):
+            L.ref_frame_set_noise_lut.argtypes = [C.c_void_p, C.c_void_p]
         L.ref_frame_get_plane.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]
         L.ref_frame_render.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_double)]
         L.ref_decode_native.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_size_t,
@@ -261,6 +271,31 @@ class Frame:
         rc = lib().ref_frame_set_params(self.h, C.byref(p))
         if rc:
             raise RuntimeError(f"ref_frame_set_params rc={rc}")
+        lib().ref_frame_info(self.h, C.byref(self.info))
+
+    def set_upsampling_weights(self, n: int, weights) -> None:
+        """Custom upsampling weights of factor n (F16 values), read into the frame's CustomTransformData through
+        the reference's Bundle reader."""
+        if not can_set_ups_noise():
+            raise RuntimeError(f"{_SO[_variant]} predates ref_frame_set_upsampling_weights: rebuild it with "
+                               "`python oracle/build_ref.py`")
+        w = np.ascontiguousarray(weights, np.float32)
+        rc = lib().ref_frame_set_upsampling_weights(self.h, n, w.ctypes.data)
+        if rc:
+            raise RuntimeError(f"ref_frame_set_upsampling_weights rc={rc}")
+        lib().ref_frame_info(self.h, C.byref(self.info))
+
+    def set_noise_lut(self, lut) -> None:
+        """The noise strength LUT (values k / 1024, k <= 1023), read through the reference's DecodeNoise; the frame
+        must carry the noise flag."""
+        if not can_set_ups_noise():
+            raise RuntimeError(f"{_SO[_variant]} predates ref_frame_set_noise_lut: rebuild it with "
+                               "`python oracle/build_ref.py`")
+        v = np.ascontiguousarray(lut, np.float32)
+        assert v.size == 8
+        rc = lib().ref_frame_set_noise_lut(self.h, v.ctypes.data)
+        if rc:
+            raise RuntimeError(f"ref_frame_set_noise_lut rc={rc}")
         lib().ref_frame_info(self.h, C.byref(self.info))
 
     def raw_group_major_coeffs(self) -> np.ndarray:

@@ -52,6 +52,8 @@
 #include "lib/jxl/dec_frame.h"
 #include "lib/jxl/dec_group.h"
 #include "lib/jxl/dec_transforms_testonly.h"
+#include "lib/jxl/enc_aux_out.h"
+#include "lib/jxl/enc_bit_writer.h"
 #include "lib/jxl/enc_transforms.h"
 #include "lib/jxl/epf.h"
 #include "lib/jxl/fields.h"
@@ -720,6 +722,75 @@ Status SetParamsImpl(RefFrame* f, const RefFrameParams& p) {
 
 REF_API int ref_frame_set_params(void* h, const RefFrameParams* p) {
   return SetParamsImpl(static_cast<RefFrame*>(h), *p) ? 0 : 1;
+}
+
+// (3c) custom upsampling weights of factor N (2, 4, 8: 15 / 55 / 210 values) as if the image header had carried
+// them: the metadata's CustomTransformData with that bit of custom_weights_mask set, written with the reference's
+// own Bundle writer and read back with Bundle::Read into the frame's transform_data, which UpsamplingStage and
+// ref_frame_info read.  Every value must be exactly F16.
+namespace {
+Status SetUpsamplingWeightsImpl(RefFrame* f, int n, const float* w) {
+  const size_t count = n == 2 ? 15 : n == 4 ? 55 : n == 8 ? 210 : 0;
+  if (!count) return JXL_FAILURE("upsampling factor");
+  for (size_t i = 0; i < count; i++) {
+    uint32_t bits;
+    if (!HalfBits(w[i], &bits)) return JXL_FAILURE("upsampling weight not F16");
+  }
+  CustomTransformData td = f->metadata.transform_data;
+  td.nonserialized_xyb_encoded = f->metadata.m.xyb_encoded;
+  const uint32_t bit = n == 2 ? 1u : n == 4 ? 2u : 4u;
+  td.custom_weights_mask |= bit;
+  float* dst = n == 2 ? td.upsampling2_weights : n == 4 ? td.upsampling4_weights : td.upsampling8_weights;
+  memcpy(dst, w, count * sizeof(float));
+  BitWriter writer(&f->mm);
+  JXL_RETURN_IF_ERROR(Bundle::Write(td, &writer, LayerType::Header, nullptr));
+  writer.ZeroPadToByte();
+  const Span<const uint8_t> span = writer.GetSpan();
+  CustomTransformData back;
+  back.nonserialized_xyb_encoded = td.nonserialized_xyb_encoded;
+  BitReader br(Bytes(span.data(), span.size()));
+  Status st = Bundle::Read(&br, &back);
+  Status closed = br.Close();
+  JXL_RETURN_IF_ERROR(st);
+  JXL_RETURN_IF_ERROR(closed);
+  const float* got = n == 2 ? back.upsampling2_weights : n == 4 ? back.upsampling4_weights : back.upsampling8_weights;
+  if (!(back.custom_weights_mask & bit) || memcmp(got, w, count * sizeof(float)))
+    return JXL_FAILURE("upsampling weights not taken");
+  f->metadata.transform_data = back;
+  return true;
+}
+
+// (3d) the noise strength LUT as the frame header's noise parameters carry it: eight 10-bit codes read by the
+// reference's DecodeNoise (lut[i] = code / 1024).  Every value must be k / 1024 with k <= 1023.
+Status SetNoiseLutImpl(RefFrame* f, const float* lut) {
+  BitPacker bits;
+  for (int i = 0; i < 8; i++) {
+    const float k = lut[i] * 1024.0f;
+    if (!(k >= 0.0f && k <= 1023.0f) || k != std::floor(k)) return JXL_FAILURE("noise LUT entry not k / 1024");
+    bits.Put(static_cast<uint32_t>(k), 10);
+  }
+  NoiseParams np;
+  BitReader br(Bytes(bits.bytes.data(), bits.bytes.size()));
+  Status st = DecodeNoise(&br, &np);
+  Status closed = br.Close();
+  JXL_RETURN_IF_ERROR(st);
+  JXL_RETURN_IF_ERROR(closed);
+  for (int i = 0; i < 8; i++)
+    if (np.lut[i] != lut[i]) return JXL_FAILURE("noise LUT not taken");
+  f->dec_state->shared_storage.image_features.noise_params = np;
+  return true;
+}
+}  // namespace
+
+REF_API int ref_frame_set_upsampling_weights(void* h, int n, const float* w) {
+  return SetUpsamplingWeightsImpl(static_cast<RefFrame*>(h), n, w) ? 0 : 1;
+}
+
+// (the frame must carry the noise flag: the encoder's photon noise sets it)
+REF_API int ref_frame_set_noise_lut(void* h, const float* lut) {
+  auto* f = static_cast<RefFrame*>(h);
+  if (!(f->frame_header->flags & FrameHeader::kNoise)) return 2;
+  return SetNoiseLutImpl(f, lut) ? 0 : 1;
 }
 
 // plane ids for ref_frame_get_plane

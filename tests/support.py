@@ -247,6 +247,309 @@ def assert_decoy_differs(decoy_px: np.ndarray, want: np.ndarray, planar: bool, m
     assert frac >= min_frac, f"the decoy matches the target on {1 - frac:.2%} of the pixels"
 
 
+# ---- upsampling and noise ----
+
+# A strength LUT of legal values (NoiseParams: 10-bit codes k / 1024, k <= 1023) that spans 0 .. 1023/1024 and is
+# not monotone, so every segment of StrengthEvalLut interpolates between different values.
+NOISE_LUT_WIDE = tuple(k / 1024 for k in (96, 1023, 410, 0, 700, 255, 880, 512))
+UPS_WEIGHT_COUNT = {2: 15, 4: 55, 8: 210}
+
+
+def default_upsampling_weights(n: int) -> np.ndarray:
+    return np.load(GOLDEN / "upsampling_weights.npz")[f"weights{n}"]
+
+
+def custom_upsampling_weights(n: int, seed: int) -> np.ndarray:
+    """Random F16 weights of factor n (CustomTransformData::upsampling{n}_weights): the defaults scaled by 0.4..1.6
+    with noise added and a tenth of the signs flipped, so no two entries of the triangular layout are related."""
+    rng = np.random.default_rng(seed)
+    d = default_upsampling_weights(n).astype(np.float64)
+    w = d * rng.uniform(0.4, 1.6, d.size) + rng.normal(0, 0.02, d.size)
+    w = np.where(rng.random(d.size) < 0.1, -w, w)
+    return wl.f16(w)
+
+
+def filter_mask(desc: abi.FrameDesc) -> int:
+    """The filter stages (Gaborish, EPF passes) of the frame's chain as stage-mask bits."""
+    if desc.stage_mask & abi.STAGE_EXPLICIT:
+        return desc.stage_mask & 15
+    return ((abi.STAGE_GAB if desc.gab else 0) | (abi.STAGE_EPF0 if desc.epf_iters >= 3 else 0) |
+            (abi.STAGE_EPF1 if desc.epf_iters >= 1 else 0) | (abi.STAGE_EPF2 if desc.epf_iters >= 2 else 0))
+
+
+def pre_upsampling_desc(desc: abi.FrameDesc) -> abi.FrameDesc:
+    """The same frame cut after its filters: planar XYB at the coded size, without upsampling and noise."""
+    import dataclasses
+    return dataclasses.replace(desc, upsampling=0, upsampling_weights=None, xsize_upsampled=0, ysize_upsampled=0,
+                               noise=0, stage_mask=abi.STAGE_EXPLICIT | filter_mask(desc),
+                               out_format=abi.OUT_PLANAR_F32)
+
+
+def out_size(desc: abi.FrameDesc) -> tuple[int, int]:
+    n = desc.upsampling if desc.upsampling > 1 else 1
+    return (desc.xsize_upsampled or n * desc.xsize, desc.ysize_upsampled or n * desc.ysize) if n > 1 \
+        else (desc.xsize, desc.ysize)
+
+
+def ups_noise_frame(n: int, w: int, h: int, seed: int, weights: str = "custom", lut=NOISE_LUT_WIDE, noise: bool = True,
+                    hdr=None, gab: int = 1, epf_iters: int = 1, fmt: int = abi.OUT_RGB_F32, srgb: int = 0,
+                    ac_type: int = abi.AC_INT16, frame_index=(3, 1)):
+    """A frame that drives the upsampling and the noise into all their branches.  n: 1 (noise only), 2, 4 or 8;
+    the output is n*w - (n-1) x n*h - 1 (ragged).  Per 8x8 block the Y DC is drawn from one of three ranges: 1.5..3
+    (AddNoise's strength saturates), -0.6..-0.05 (below X: negative input, clamped to the LUT's start) or 0..1.5
+    (every LUT segment); independent block DCs make hard edges, where the upsampler's window clamp engages.
+    `weights`: "custom" (random F16, custom_upsampling_weights) or "default"; `hdr`: a jxl_workload.header_params
+    name or seed (header_frame)."""
+    if hdr is not None:
+        desc, coeffs = header_frame(w, h, seed, hdr, gab=gab, epf_iters=epf_iters, ac_type=ac_type)
+    else:
+        desc, coeffs = wl.synthetic_frame(w, h, seed=seed, gab=gab, epf_iters=epf_iters, ac_type=ac_type)
+    rng = np.random.default_rng(seed + 515)
+    shape = desc.dc.shape[1:]
+    kind = rng.integers(0, 3, shape)
+    y = np.where(kind == 0, rng.uniform(1.5, 3.0, shape), np.where(kind == 1, rng.uniform(-0.6, -0.05, shape),
+                                                                   rng.uniform(0.0, 1.5, shape)))
+    desc.dc = desc.dc.copy()
+    desc.dc[1] = y.astype(np.float32)
+    if n > 1:
+        desc.upsampling = n
+        desc.upsampling_weights = (custom_upsampling_weights(n, seed) if weights == "custom"
+                                   else default_upsampling_weights(n))
+        desc.xsize_upsampled, desc.ysize_upsampled = n * w - (n - 1), n * h - 1
+    if noise:
+        desc.noise, desc.noise_lut = 1, tuple(lut)
+        desc.visible_frame_index, desc.nonvisible_frame_index = frame_index
+    desc.out_format, desc.stage_mask = fmt, srgb
+    return desc, coeffs
+
+
+def ups_decoy(desc: abi.FrameDesc, seed: int):
+    """A frame of the same geometry, chain and output as the upsampled / noisy `desc` with other content, other
+    frame indices (other noise) and other weights.  Rendered on a context just before `desc` it leaves ups_in,
+    noise_raw, noise_buf and the tap table full of values that are wrong for `desc`."""
+    import dataclasses
+    d, coeffs = decoy_frame(desc, seed)
+    n = desc.upsampling if desc.upsampling > 1 else 1
+    # the frame's X, Y and B DC mirrored: where the frame saturates an 8-bit channel, the decoy does not
+    dc = np.stack([-desc.dc[0], np.float32(1.4) - desc.dc[1], np.float32(0.6) - desc.dc[2]]).astype(np.float32)
+    d = dataclasses.replace(d, dc=dc, visible_frame_index=desc.visible_frame_index + 7,
+                            nonvisible_frame_index=desc.nonvisible_frame_index + 11)
+    if n > 1:
+        d.upsampling_weights = custom_upsampling_weights(n, seed + 1)
+    return d, coeffs
+
+
+def mirror_index(i: np.ndarray, size: int) -> np.ndarray:
+    """Mirror() of image_ops.h: reflect (edge repeated) until inside [0, size)."""
+    i = np.asarray(i, np.int64).copy()
+    while True:
+        lo, hi = i < 0, i >= size
+        if not (lo.any() or hi.any()):
+            return i
+        i = np.where(lo, -i - 1, np.where(hi, 2 * size - 1 - i, i))
+
+
+def tap_table(weights, n: int, transpose: bool = False) -> np.ndarray:
+    """(n, n, 5, 5) float64 taps of output sub-pixel (ky, kx), built from the n/2 x n/2 x 25 weights as the symmetric
+    (5n/2)^2 matrix whose upper triangle they list row by row: sub-pixels in the lower / right half use the mirrored
+    sub-pixel and the mirrored window.  transpose: each 5x5 transposed (a deliberately wrong model)."""
+    h = n // 2
+    m = 5 * h
+    w = np.asarray(weights, np.float64)
+    assert w.size == m * (m + 1) // 2
+    M = np.zeros((m, m))
+    iu = np.triu_indices(m)
+    M[iu] = w
+    M[iu[1], iu[0]] = w
+    t = np.zeros((n, n, 5, 5))
+    for ky in range(n):
+        for kx in range(n):
+            fy, fx = ky if ky < h else n - 1 - ky, kx if kx < h else n - 1 - kx
+            for py in range(5):
+                for px in range(5):
+                    j = 5 * fy + (py if ky < h else 4 - py)
+                    i = 5 * fx + (px if kx < h else 4 - px)
+                    t[ky, kx, py, px] = M[j, i]
+    return t.transpose(0, 1, 3, 2).copy() if transpose else t
+
+
+def upsample_model(planes: np.ndarray, weights, n: int, ow: int, oh: int, clamp: bool = True,
+                   transpose: bool = False):
+    """float64 UpsamplingStage: (3, h, w) planes -> (out, unclamped, sum|v*k|), each (3, oh, ow).  Input mirrored about
+    the coded size; every output clamped to the min / max of its 5x5 input window."""
+    c, h, w = planes.shape
+    p = planes.astype(np.float64)
+    ys, xs = mirror_index(np.arange(-2, h + 2), h), mirror_index(np.arange(-2, w + 2), w)
+    pad = p[:, ys][:, :, xs]
+    win = np.lib.stride_tricks.sliding_window_view(pad, (5, 5), axis=(1, 2))     # (3, h, w, 5, 5)
+    mn, mx = win.min(axis=(3, 4)), win.max(axis=(3, 4))
+    taps = tap_table(weights, n, transpose)
+    raw = np.zeros((c, h * n, w * n))
+    acc = np.zeros_like(raw)
+    out = np.zeros_like(raw)
+    for ky in range(n):
+        for kx in range(n):
+            k = taps[ky, kx]
+            r = np.einsum("chwij,ij->chw", win, k)
+            raw[:, ky::n, kx::n] = r
+            acc[:, ky::n, kx::n] = np.einsum("chwij,ij->chw", np.abs(win), np.abs(k))
+            out[:, ky::n, kx::n] = np.clip(r, mn, mx) if clamp else r
+    return out[:, :oh, :ow], raw[:, :oh, :ow], acc[:, :oh, :ow]
+
+
+def convolve_noise_model(raw: np.ndarray, mirror_wh=None):
+    """float64 ConvolveNoiseStage of (3, H, W) generator planes: 0.16 * (sum of the 24 neighbours) - 3.84 * centre,
+    borders mirrored about the output size (`mirror_wh`: about another size, a deliberately wrong model).
+    Returns (conv, 0.16 * others + 3.84 * |centre| for the error bound)."""
+    _, H, W = raw.shape
+    mw, mh = mirror_wh or (W, H)
+    r = raw.astype(np.float64)
+    xs = [mirror_index(np.arange(W) + d, mw) for d in range(-2, 3)]
+    ys = [mirror_index(np.arange(H) + d, mh) for d in range(-2, 3)]
+    others = np.zeros_like(r)
+    for dy in range(5):
+        for dx in range(5):
+            if dy != 2 or dx != 2:
+                others += r[:, ys[dy]][:, :, xs[dx]]
+    centre = r[:, ys[2]][:, :, xs[2]]
+    return 0.16 * others - 3.84 * centre, 0.16 * others + 3.84 * np.abs(centre)
+
+
+def noise_strength_model(lut, x: np.ndarray) -> np.ndarray:
+    """StrengthEvalLut in float64."""
+    lut = np.asarray(lut, np.float64)
+    s = np.maximum(x * 6.0, 0.0)
+    fl = np.floor(s)
+    frac = s - fl
+    sat = s >= 7.0
+    fl, frac = np.where(sat, 6.0, fl), np.where(sat, 1.0, frac)
+    i = fl.astype(np.int64)
+    return np.clip(lut[i] + (lut[i + 1] - lut[i]) * frac, 0.0, 1.0)
+
+
+def lut_segments(x: np.ndarray) -> np.ndarray:
+    """Which branch of StrengthEvalLut an input takes: -1 negative (clamped to 0), 0..6 the segment, 7 saturated."""
+    s = x * 6.0
+    return np.where(s < 0, -1, np.where(s >= 7.0, 7, np.floor(np.maximum(s, 0)))).astype(np.int64)
+
+
+def add_noise_model(xyb: np.ndarray, conv: np.ndarray, lut, cfl_x: float, cfl_b: float) -> np.ndarray:
+    """float64 AddNoiseStage on (3, H, W) X, Y, B with the convolved noise planes."""
+    X, Y, B = xyb
+    rr, rg, rc = conv * 0.22
+    sg, sr = noise_strength_model(lut, (Y - X) * 0.5), noise_strength_model(lut, (Y + X) * 0.5)
+    red = sr * (0.0078125 * rr + 0.9921875 * rc)
+    green = sg * (0.0078125 * rg + 0.9921875 * rc)
+    s = red + green
+    return np.stack([cfl_x * s + (red - green) + X, Y + s, cfl_b * s + B])
+
+
+def ups_noise_coverage(desc: abi.FrameDesc, coeffs: np.ndarray, what: str = "", pre: np.ndarray | None = None,
+                       min_segment: int = 100) -> dict:
+    """What the frame exercises, in float64 from the oracle's pre-upsampling planes (`pre`: those planes if at hand):
+    the fraction of output samples per channel that the window clamp changed (at least 1 %, and some in the ragged
+    last 256-tile of every tile row and tile column), the number of AddNoise inputs (Y - X and Y + X) per branch of
+    StrengthEvalLut (every one at least `min_segment`) and the output's raggedness.  Prints and returns the figures."""
+    from oracle import cpu as ocpu
+    if pre is None:
+        pre = ocpu.render_frame(pre_upsampling_desc(desc), coeffs, rcp_mode=0)
+    n = desc.upsampling if desc.upsampling > 1 else 1
+    ow, oh = out_size(desc)
+    res = {"out": (ow, oh)}
+    assert ow % 256 and oh % 256, ("no ragged 256-tile", ow, oh)
+    if n > 1:
+        xyb, raw, _ = upsample_model(pre, desc.upsampling_weights, n, ow, oh)
+        changed = xyb != raw
+        res["clamp_frac"] = [float(changed[c].mean()) for c in range(3)]
+        tx, ty = (ow // 256) * 256, (oh // 256) * 256
+        right = [bool(changed[:, y0:y0 + 256, tx:].any()) for y0 in range(0, oh, 256)]
+        bottom = [bool(changed[:, ty:, x0:x0 + 256].any()) for x0 in range(0, ow, 256)]
+        assert min(res["clamp_frac"]) >= 0.01, (what, res["clamp_frac"])
+        assert all(right) and all(bottom), (what, right, bottom)
+    else:
+        xyb = pre.astype(np.float64)
+    if desc.noise:
+        seg = np.concatenate([lut_segments((xyb[1] - xyb[0]) * 0.5).ravel(),
+                              lut_segments((xyb[1] + xyb[0]) * 0.5).ravel()])
+        counts = np.bincount(seg + 1, minlength=9)
+        res["lut_counts"] = {"neg": int(counts[0]), **{str(i): int(counts[i + 1]) for i in range(7)},
+                             "sat": int(counts[8])}
+        assert counts.min() >= min_segment, (what, res["lut_counts"])
+    print(f"coverage {what}: {n}x, output {ow}x{oh} (w % 16 = {ow % 16}, last tile {ow % 256}x{oh % 256}); "
+          f"clamp fraction per channel {[f'{v:.2%}' for v in res.get('clamp_frac', [])]}; "
+          f"LUT branches {res.get('lut_counts')}")
+    return res
+
+
+GAMMA_25 = 25 * 2.0 ** -24 / (1 - 25 * 2.0 ** -24)   # Higham's gamma_n: n float32 roundings in a row
+
+
+def check_float64_model(p, desc: abi.FrameDesc, coeffs: np.ndarray, what: str = "") -> dict:
+    """Render `desc` on the pipeline `p` as planar XYB (no colour stage) and compare it with the float64 models of
+    the upsampling (from the n/2 triangular weights, not the kernel's table), ConvolveNoise and AddNoise, fed with
+    the kernels' own pre-upsampling planes (a render of pre_upsampling_desc) and the oracle's generator planes.  The
+    bound is counted per sample from the float32 operations (u = 2^-24 per rounding).  Asserts that the largest
+    error is within it and, for upsampled frames, that three wrong models (5x5 taps transposed, no window clamp,
+    noise mirrored about the coded size) exceed it at least 100 times.  Prints and returns the ratios."""
+    import dataclasses
+    from oracle import cpu as ocpu
+    pre = p.decode_frame(pre_upsampling_desc(desc), coeffs)
+    d = dataclasses.replace(desc, stage_mask=abi.STAGE_EXPLICIT | filter_mask(desc), out_format=abi.OUT_PLANAR_F32)
+    got = p.decode_frame(d, coeffs).astype(np.float64)
+    n = desc.upsampling if desc.upsampling > 1 else 1
+    ow, oh = out_size(desc)
+    u = 2.0 ** -24
+    gen = ocpu.noise_planes(desc.visible_frame_index, desc.nonvisible_frame_index, ow, oh) if desc.noise else None
+    lut = np.asarray(desc.noise_lut, np.float64)
+    slope = 3.0 * np.abs(np.diff(lut)).max()      # d strength / d input (x * 0.5 * 6)
+
+    def model(transpose=False, clamp=True, mirror=None):
+        if n > 1:
+            up, _, acc = upsample_model(pre, desc.upsampling_weights, n, ow, oh, clamp, transpose)
+        else:
+            up, acc = pre.astype(np.float64), np.zeros((3, oh, ow))
+        e_up = GAMMA_25 * acc + u * np.abs(up)      # 25 products summed in any order, then the clamp
+        if not desc.noise:
+            return up, e_up + u * np.abs(up)
+        conv, cmag = convolve_noise_model(gen, mirror)
+        out = add_noise_model(up, conv, lut, desc.cfl_base_x, desc.cfl_base_b)
+        X, Y, _ = up
+        rnd = 0.22 * conv
+        e_rnd = 0.22 * 30 * u * cmag + u * np.abs(rnd)
+        m_r = 0.0078125 * rnd[0] + 0.9921875 * rnd[2]
+        m_g = 0.0078125 * rnd[1] + 0.9921875 * rnd[2]
+        e_mr = 0.0078125 * e_rnd[0] + 0.9921875 * e_rnd[2] + 2 * u * (np.abs(rnd[0]) + np.abs(rnd[2]))
+        e_mg = 0.0078125 * e_rnd[1] + 0.9921875 * e_rnd[2] + 2 * u * (np.abs(rnd[1]) + np.abs(rnd[2]))
+        e_s = slope * (e_up[0] + e_up[1] + 3 * u * (np.abs(X) + np.abs(Y))) + 4 * u
+        sr = noise_strength_model(lut, (Y + X) * 0.5)
+        sg = noise_strength_model(lut, (Y - X) * 0.5)
+        red, green = sr * m_r, sg * m_g
+        e_red = e_s * np.abs(m_r) + sr * e_mr + u * np.abs(red)
+        e_green = e_s * np.abs(m_g) + sg * e_mg + u * np.abs(green)
+        s = red + green
+        e_sum = e_red + e_green + u * np.abs(s)
+        cx, cb = abs(desc.cfl_base_x), abs(desc.cfl_base_b)
+        bound = np.stack([
+            e_up[0] + cx * e_sum + e_red + e_green + 3 * u * (cx * np.abs(s) + np.abs(red) + np.abs(green) + np.abs(out[0])),
+            e_up[1] + e_sum + u * np.abs(out[1]),
+            e_up[2] + cb * e_sum + 2 * u * (cb * np.abs(s) + np.abs(out[2]))])
+        return out, bound
+
+    want, bound = model()
+    ratio = float((np.abs(got - want) / bound).max())
+    res = {"ratio": ratio}
+    if n > 1:
+        wrong = {"transposed taps": model(transpose=True)[0], "no clamp": model(clamp=False)[0]}
+        if desc.noise:
+            wrong["noise mirrored about the coded size"] = model(mirror=(desc.xsize, desc.ysize))[0]
+        res.update({k: float((np.abs(got - v) / bound).max()) for k, v in wrong.items()})
+    print(f"float64 model {what}: largest error {ratio:.3g} of the bound; wrong models: "
+          f"{ {k: f'{v:.3g}' for k, v in res.items() if k != 'ratio'} }")
+    assert ratio <= 1.0, (what, ratio)
+    assert all(v >= 100 for k, v in res.items() if k != "ratio"), (what, res)
+    return res
+
+
 def dc_stage_input(xs: int, ys: int) -> np.ndarray:
     """Seeded quantised DC planes (X, Y, B): smooth gradients (adaptive smoothing engages) with one busy
     quadrant (it must switch itself off there)."""

@@ -322,6 +322,68 @@ def test_noise_stages_bit_exact(rs, w, h, iso, hdr, refmod):
         assert np.array_equal(np.moveaxis(want, 0, 2), refmod.decode_linear_f32(data, 2))
 
 
+def need_ups_noise_setters(refmod):
+    """Frame.set_upsampling_weights / set_noise_lut; a harness prebuilt without them is a skip only where the
+    reference sources are not there to rebuild it."""
+    import os
+    if not refmod.can_set_ups_noise():
+        if os.path.isdir(os.environ.get("JXL_REFERENCE_ROOT", "/root/reference")):
+            pytest.fail("oracle/_ref predates ref_frame_set_upsampling_weights / ref_frame_set_noise_lut although the "
+                        "reference is present: run `python oracle/build_ref.py`")
+        pytest.skip("oracle/_ref was built from a harness without ref_frame_set_upsampling_weights")
+
+
+@pytest.mark.parametrize("rs,w,h,noise,hdr", [(2, 601, 299, False, None), (4, 1101, 517, False, None),
+                                              (8, 2101, 167, False, None), (4, 1101, 517, True, None),
+                                              (8, 2101, 167, True, None), (8, 2101, 167, True, "edges")])
+def test_custom_weights_and_noise_lut_bit_exact(rs, w, h, noise, hdr, refmod):
+    """Random F16 upsampling weights (negative ones, no two entries of the triangular layout related:
+    support.custom_upsampling_weights) read into the reference's CustomTransformData through its Bundle reader, and
+    the wide non-monotone LUT (support.NOISE_LUT_WIDE, up to 1023/1024) through its DecodeNoise.  Output sizes are
+    multiples of neither N nor 16 nor 256, so noise tiles and the upsampler's mirror are ragged.  The oracle is
+    bit-exact against the reference's own stages, with and without the colour stage; the weights really are the
+    custom ones (the render differs from the default weights')."""
+    import dataclasses
+    from oracle import cpu
+    need_ups_noise_setters(refmod)
+    img = wl.synth_image(w, h, seed=rs + 7)
+    data = refmod.encode_rgb8(img, 1.0, 7, -1, -1, 4, resampling=rs | ((6400 // 100) << 16 if noise else 0))
+    fr = refmod.Frame(data, 2)
+    if hdr is not None:
+        set_header(refmod, fr, hdr)
+    wts = support.custom_upsampling_weights(rs, seed=rs + (1 if noise else 0))
+    fr.set_upsampling_weights(rs, wts)
+    if noise:
+        fr.set_noise_lut(support.NOISE_LUT_WIDE)
+    i = fr.info
+    assert i.upsampling == rs and (i.xsize_upsampled, i.ysize_upsampled) == (w, h) and i.noise == int(noise)
+    assert np.array_equal(np.float32(list(i.upsampling_weights)[:support.UPS_WEIGHT_COUNT[rs]]), wts)
+    if noise:
+        assert np.array_equal(np.float32(list(i.noise_lut)), np.float32(support.NOISE_LUT_WIDE))
+    d = fr.dump()
+    desc = cpu.desc_from_dump(d)
+    desc.out_format = abi.OUT_PLANAR_F32
+    chain = (1 if i.gab else 0) | (2 if i.epf_iters >= 3 else 0) | (4 if i.epf_iters >= 1 else 0) | (8 if i.epf_iters >= 2 else 0)
+    stages = refmod.STAGE_UPSAMPLING | (refmod.STAGE_NOISE if noise else 0)
+    want, _ = fr.render(chain | refmod.STAGE_XYB | stages)
+    assert want.shape == (3, h, w)
+    got = cpu.render_frame(desc, d.coeffs, rcp_mode=1)
+    assert np.array_equal(got, want)
+    desc.stage_mask = abi.STAGE_EXPLICIT | chain          # the upsampled (noisy) XYB planes themselves
+    want_xyb, _ = fr.render(chain | stages)
+    assert np.array_equal(cpu.render_frame(desc, d.coeffs, rcp_mode=1), want_xyb)
+    ups_xyb, _ = fr.render(chain | refmod.STAGE_UPSAMPLING)
+    fr.close()
+    default = dataclasses.replace(desc, upsampling_weights=support.default_upsampling_weights(rs), noise=0)
+    assert not np.array_equal(cpu.render_frame(default, d.coeffs, rcp_mode=1), ups_xyb)
+    if noise:   # what AddNoise sees: content of an 8-bit sRGB image keeps Y +- X below 7/3, short of saturation
+        X, Y = ups_xyb[0].astype(np.float64), ups_xyb[1].astype(np.float64)
+        seg = np.concatenate([support.lut_segments((Y - X) * 0.5).ravel(), support.lut_segments((Y + X) * 0.5).ravel()])
+        counts = np.bincount(seg + 1, minlength=9)
+        print(f"{rs}x {w}x{h}: AddNoise inputs per LUT branch (negative, segments 0..6, saturated): {counts.tolist()}")
+        assert (counts[1:4] >= 100).all(), counts
+
+
 def make_jpeg(w, h, quality, seed=5):
     """A baseline 4:4:4 JPEG of the seeded test image (Pillow)."""
     import io
