@@ -2523,6 +2523,28 @@ __device__ __forceinline__ void filter_strip_body(const FrameDev& P, char* __res
     pre_b = ldg_xyb(P.xyb + P.plane_stride + off);
     pre_c = ldg_xyb(P.xyb + 2 * P.plane_stride + off);
   }
+  // Gaborish window.  Gaborish's sums are h(T) + h(B) and h(M) + (T[t] + B[t]) with h(row) = row[x-1] + row[x+1],
+  // so each row's h is used three times: as B, as M, then as T.  The window keeps h(T) and h(M) of each channel in
+  // registers, and a windowed step reads only its new row's h(B) (plus T[t], M[t], B[t]) from the ring: 15 shared
+  // loads instead of 27.  Same operations in the same order, so the same bits.  It is filled from the ring where
+  // the windowed steps begin (the steps before may mirror rows) and carried through the 8x unrolled steady steps
+  // only, or through every steady step of the EPF0 chains, whose register budget is twice as large: with 64
+  // registers, carrying it through the unaligned steady steps as well spills there.  (Keeping T[t], M[t], B[t] in
+  // registers as well would save 9 more loads but spills inside the unrolled steps.)
+  float gwh[2][3];
+  auto prime_window = [&](int rin) {
+    if constexpr (C::G) {
+      const float* pT0 = ring_row(ringG, C::NG, rin - dG - 1, 0);
+      const float* pM0 = ring_row(ringG, C::NG, rin - dG, 0);
+#pragma unroll
+      for (int c = 0; c < 3; c++) {
+        const float* pT = pT0 + c * kStripThreads;
+        const float* pM = pM0 + c * kStripThreads;
+        gwh[0][c] = pT[cn[2]] + pT[cn[4]];
+        gwh[1][c] = pM[cn[2]] + pM[cn[4]];
+      }
+    }
+  };
 
   // inverse sigma of each EPF stage's next row, fetched one step ahead as well.  A stage's first
   // produced row is max(0, y_begin - rem) (its `lo`), reached at step lo + delay.
@@ -2645,9 +2667,18 @@ __device__ __forceinline__ void filter_strip_body(const FrameDev& P, char* __res
           const float* pT = pT0 + c * kStripThreads;
           const float* pM = pM0 + c * kStripThreads;
           const float* pB = pB0 + c * kStripThreads;
-          const float sum1 = (pM[cn[2]] + pM[cn[4]]) + (pT[t] + pB[t]);
-          const float sum2 = (pT[cn[2]] + pT[cn[4]]) + (pB[cn[2]] + pB[cn[4]]);
-          v[c] = fmaf(sum2, P.gab_w[3 * c + 2], fmaf(sum1, P.gab_w[3 * c + 1], pM[t] * P.gab_w[3 * c]));
+          if constexpr (ST && (J >= 0 || C::E0)) {  // the window holds h(T), h(M) (see prime_window)
+            const float hB = pB[cn[2]] + pB[cn[4]];
+            const float sum1 = gwh[1][c] + (pT[t] + pB[t]);
+            const float sum2 = gwh[0][c] + hB;
+            v[c] = fmaf(sum2, P.gab_w[3 * c + 2], fmaf(sum1, P.gab_w[3 * c + 1], pM[t] * P.gab_w[3 * c]));
+            gwh[0][c] = gwh[1][c];
+            gwh[1][c] = hB;
+          } else {
+            const float sum1 = (pM[cn[2]] + pM[cn[4]]) + (pT[t] + pB[t]);
+            const float sum2 = (pT[cn[2]] + pT[cn[4]]) + (pB[cn[2]] + pB[cn[4]]);
+            v[c] = fmaf(sum2, P.gab_w[3 * c + 2], fmaf(sum1, P.gab_w[3 * c + 1], pM[t] * P.gab_w[3 * c]));
+          }
         }
         deliver(IC<1>(), r, t, v[0], v[1], v[2]);
       }
@@ -2896,6 +2927,9 @@ __device__ __forceinline__ void filter_strip_body(const FrameDev& P, char* __res
   };
   int rin = r_in_lo;
   for (; rin < s_begin; rin++) step(F(), IC<-1>(), rin);
+  if constexpr (C::E0) {
+    if (rin < s_end) prime_window(rin);
+  }
   if constexpr (H > 0 && !C::E0) {
     // 8x unrolled steady loop with compile-time ring slots (EPF0 chains are too large to replicate)
     if (C::kCompact && rin < s_end) {  // (an unaligned step loads every pass's block selection: the aligned
@@ -2903,6 +2937,7 @@ __device__ __forceinline__ void filter_strip_body(const FrameDev& P, char* __res
       rin++;
     }
     for (; rin < s_end && (rin & 7); rin++) step(T(), IC<-1>(), rin);
+    if (rin + 8 <= s_end) prime_window(rin);
     for (; rin + 8 <= s_end; rin += 8) {
       step(T(), IC<0>(), rin);
       step(T(), IC<1>(), rin + 1);
