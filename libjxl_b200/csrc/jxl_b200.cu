@@ -232,7 +232,7 @@ int launch_idct(jxlgpu_ctx* ctx, uint32_t row0, uint32_t row1, uint32_t need_y0,
   const bool prof = ctx->profile;
   const bool fused = use_fused(ctx);
   P.fused = fused ? 1u : 0u;
-  CU(cudaMemsetAsync(ctx->counts.p, 0, kNumStrategies * sizeof(uint32_t), s));
+  CU(cudaMemsetAsync(ctx->counts.p, 0, kCountWords * sizeof(uint32_t), s));  // (the 8x8 kernel's work counter too)
   const int want_sigma = (P.stage_mask & 14u) ? 1 : 0;
   if (prof) CU(cudaEventRecord(ctx->prof_ev[0], s));
   plan_kernel<<<plan_groups, 1024, 0, s>>>(P, want_sigma);
@@ -283,7 +283,12 @@ int launch_idct(jxlgpu_ctx* ctx, uint32_t row0, uint32_t row1, uint32_t need_y0,
     idct_large_kernel<false, 1><<<grid_large, kLargeWarps * 32, kLargeSmem, sl>>>(P);
   }
   if (prof) CU(cudaEventRecord(ctx->prof_ev[4], s));
-  if (!prof) run8();  // after the (usually tiny) side kernels grabbed their few SM slots
+  // The side kernels go first: launched after it, they would find every SM full of 8x8 CTAs and start only as
+  // those finish (where they have real work, e.g. all-27-strategy frames, they are the longer chain).  While one of
+  // their CTAs is resident (mid: 126 registers x 256 threads, large: 107 KB of shared memory), its SM holds one 8x8
+  // CTA instead of two; the 8x8 kernel's warps claim their items from a counter, so the CTAs that start late just
+  // do fewer (DESIGN.md §4, item 2).
+  if (!prof) run8();
   if (!prof) {
     CU(cudaEventRecord(ctx->ev_mid, sm));
     CU(cudaEventRecord(ctx->ev_large, sl));
@@ -528,7 +533,7 @@ int jxlgpu_create(jxlgpu_ctx** out, const jxlgpu_config* cfg) {
     ctx->launch_bytes = kLaunchBytes;
     if (const char* mb = getenv("JXLGPU_LAUNCH_MB")) ctx->launch_bytes = (size_t)atoi(mb) << 20;
   }
-  if ((e = ctx->counts.ensure(kNumStrategies * sizeof(uint32_t))) != cudaSuccess) return bail(e, "alloc");
+  if ((e = ctx->counts.ensure(kCountWords * sizeof(uint32_t))) != cudaSuccess) return bail(e, "alloc");
   for (auto& ev : ctx->prof_ev)
     if ((e = cudaEventCreate(&ev)) != cudaSuccess) return bail(e, "event");
   *out = ctx;

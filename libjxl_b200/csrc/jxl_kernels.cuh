@@ -56,6 +56,7 @@ namespace jxlb {
 constexpr float kSqrt2 = 1.41421356237f;  // lib/jxl/dct_scales.h:15
 constexpr int kNumStrategies = 27;
 constexpr int kFirstLarge = 18;           // strategies >= 18 have a 64+ side
+constexpr int kCountWords = kNumStrategies + 1;  // FrameDev::counts, zeroed before every plan launch
 
 // AcStrategy geometry (lib/jxl/ac_strategy.h:148-173): blocks covered per side.  The device functions read the
 // log2 of a side from immediates, one nibble per strategy (strategies 0..15 in the first word, 16..26 in the
@@ -112,7 +113,7 @@ struct FrameDev {
   // produced by the plan kernel
   float* sigma;              // [yb][xb] inverse sigma
   uint4* list;               // work lists: {(aby<<16)|abx, coefficient base / 64, raw quant, ytox | ytob<<8}
-  uint32_t* counts;          // [27]
+  uint32_t* counts;          // [kCountWords]: the 27 list sizes, then idct8_tma_kernel's work counter
   uint32_t list_base[kNumStrategies];
   // fused path (jxl_fused.cuh): one 16-byte record per 8x8 block, [yb][xb]:
   //   {kind (strategy 0..17 of an 8x8-class varblock | kBmapCopy), coefficient base / 64, raw quant, ytox | ytob<<8}
@@ -1187,12 +1188,16 @@ __global__ void __launch_bounds__(kSmallWarpsPerCta * 32, 4) idct8_kernel(const 
 // values two items ahead (with the copies, by three otherwise idle lanes, handed over by shuffle), the list
 // sizes sit in shared memory.  2 CTAs x 16 warps per SM (64 registers without spills, 112 KB of shared memory
 // per CTA) keep 32 warps and ~100 KB of coefficient reads in flight per SM.
+// Warps claim their items from a counter (counts[kNumStrategies]) rather than taking a fixed share: the mid and
+// large transforms run beside this kernel and hold SM slots for a while, so some of its CTAs start late, and with a
+// fixed share the kernel ended when those finished theirs.
 // Needs 16-byte aligned coefficient planes (jxlgpu_set_device_coefficients may bring others: idct8_kernel).
 // ---------------------------------------------------------------------------
 constexpr int kTma8Warps = 16;
+constexpr uint32_t kTma8Chunk = 2;  // items per claim (a power of two)
 constexpr int kTma8BlockWords = 200;  // 3 channels x 64 int32 (int16: half used) + 8: the four blocks of a warp start 8 banks apart
 constexpr int kTma8StageWords = 4 * kTma8BlockWords;
-constexpr int kTma8WarpWords = 2 * kTma8StageWords + 4;        // 2 stages | 2 mbarriers
+constexpr int kTma8WarpWords = 2 * kTma8StageWords + 8;        // 2 stages | 2 mbarriers | item ring (4)
 constexpr size_t kTma8SmemBytes = (size_t)kTma8Warps * kTma8WarpWords * 4;
 
 template <bool I32>
@@ -1200,6 +1205,7 @@ __global__ void __launch_bounds__(kTma8Warps * 32, 2) idct8_tma_kernel(const __g
   extern __shared__ __align__(16) float fsm[];
   uint32_t* wsm = reinterpret_cast<uint32_t*>(fsm) + (threadIdx.x >> 5) * kTma8WarpWords;
   uint64_t* bars = reinterpret_cast<uint64_t*>(wsm + 2 * kTma8StageWords);
+  uint32_t* ring_item = wsm + 2 * kTma8StageWords + 4;  // the item of each position of the record ring (below)
   const int lane = threadIdx.x & 31, slot = lane >> 3, l = lane & 7;
   const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
@@ -1260,6 +1266,7 @@ __global__ void __launch_bounds__(kTma8Warps * 32, 2) idct8_tma_kernel(const __g
   const uint4 zero = make_uint4(0, 0, 1, 0);
   auto fetch_rec = [&](uint32_t v, int pos) {
     const int oi = list_of(v);
+    if (lane == 0) ring_item[pos] = v;
     if (l == 6) {
       if (is_act(v, oi)) async_copy16(recs + pos * 4 + slot, P.list + P.list_base[skind[oi]] + (v - pre[oi]) * 4 + slot);
       else recs[pos * 4 + slot] = zero;
@@ -1285,23 +1292,46 @@ __global__ void __launch_bounds__(kTma8Warps * 32, 2) idct8_tma_kernel(const __g
       dc = __ldg(P.dc + (size_t)(l - 3) * P.yb * P.xb + (size_t)(rec.x >> 16) * P.xb + (rec.x & 0xffffu));
   };
 
-  uint32_t v = warp;
+  // A warp's items come in chunks of kTma8Chunk consecutive items.  Its first two chunks are fixed (items
+  // kTma8Chunk * warp and kTma8Chunk * (nwarps + warp) on), so that the launch does not begin with a burst of
+  // atomics on one address; every later chunk is claimed from the counter when its first item is fetched, three
+  // items before it is transformed.  A warp's items increase, and it stops at the first one past the end: every
+  // item below `total` is transformed exactly once.
+  uint32_t next = kTma8Chunk * warp;  // the warp's next item
+  auto claim = [&]() {
+    const uint32_t v = next++;
+    if (next % kTma8Chunk == 0) {
+      if (next == kTma8Chunk * (warp + 1)) {
+        next = kTma8Chunk * (nwarps + warp);
+      } else {
+        uint32_t c = 0;
+        if (lane == 0) c = atomicAdd(P.counts + kNumStrategies, kTma8Chunk);
+        next = 2 * kTma8Chunk * nwarps + __shfl_sync(0xffffffffu, c, 0);
+      }
+    }
+    return v;
+  };
   float dc_cur = 0.0f, dc_next = 0.0f;  // lanes 3..5: DC value l - 3 of this item's / the next item's block
-  fetch_rec(v, 0);
-  fetch_rec(v + nwarps, 1);
-  fetch_rec(v + 2 * nwarps, 2);
-  async_wait<0>();
-  __syncwarp();
-  issue(0, 0, is_act(v, list_of(v)), dc_cur);
-  issue(1, 1, is_act(v + nwarps, list_of(v + nwarps)), dc_next);
-  // ring position of item v: its staging buffer is st = pos & 1, whose completion of this item has
+  {
+    const uint32_t v0 = claim();
+    fetch_rec(v0, 0);
+    const uint32_t v1 = claim();
+    fetch_rec(v1, 1);
+    fetch_rec(claim(), 2);
+    async_wait<0>();
+    __syncwarp();
+    issue(0, 0, is_act(v0, list_of(v0)), dc_cur);
+    issue(1, 1, is_act(v1, list_of(v1)), dc_next);
+  }
+  // ring position of the current item: its staging buffer is st = pos & 1, whose completion of this item has
   // parity (pos >> 1) & 1 (each buffer takes every other item)
-  uint32_t pos = 0;
 #pragma unroll 1
-  for (; v < total; v += nwarps, pos = (pos + 1) & 3u) {
+  for (uint32_t pos = 0;; pos = (pos + 1) & 3u) {
+    const uint32_t v = ring_item[pos];
+    if (v >= total) break;
     const int st = pos & 1;
     // the record of the item three ahead starts its trip now; it is used (for the copies) next iteration
-    fetch_rec(v + 3 * nwarps, (pos + 3) & 3u);
+    fetch_rec(claim(), (pos + 3) & 3u);
     const int oi_cur = list_of(v);
     const bool act_cur = is_act(v, oi_cur);
     const int kind = skind[oi_cur];
@@ -1341,7 +1371,8 @@ __global__ void __launch_bounds__(kTma8Warps * 32, 2) idct8_tma_kernel(const __g
     async_wait<1>();
     __syncwarp();
     dc_cur = dc_next;
-    issue(st, (pos + 2) & 3u, is_act(v + 2 * nwarps, list_of(v + 2 * nwarps)), dc_next);
+    const uint32_t v2 = ring_item[(pos + 2) & 3u];
+    issue(st, (pos + 2) & 3u, is_act(v2, list_of(v2)), dc_next);
   }
 }
 
